@@ -45,6 +45,8 @@ NET_CFG = dict(_target_="neddf.network.NeDDF", embed_pos_rank=10, embed_dir_rank
 RENDER_CFG = dict(sample_coarse=S_COARSE, sample_fine=S_FINE, dist_near=2.0, dist_far=6.0, max_dist=6.0,
                   use_coarse_network=False, sampling_type="cone")
 WEIGHT_SEED = 3408
+H100_FP16_TFLOPS = 989.0  # NVIDIA H100 SXM data sheet, dense FP16 / BF16 (700 W card)
+DUMP_MAX_BYTES = 64 * 2 ** 20
 
 
 def synthetic_pose(seed: int):
@@ -92,7 +94,7 @@ def seeded_state_dict():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -139,6 +141,32 @@ class ClockSampler:
         sm.sort()
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": smax, "reasons": sorted(reasons),
                 "samples": len(sm)}
+
+
+def dump_outputs(out_dir, arrays):
+    """--dump-outputs: every array as out_dir/<name>.npy in float32 (float64 stays float64), DUMP_MAX_BYTES in all.
+    An array that does not fit the budget left is replaced by a fixed, seeded sample of its rows (the same rows in
+    every run), written with the row indices (float64) as <name>_sample_rows.npy; both count against the budget."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    budget = DUMP_MAX_BYTES
+    names = list(arrays)
+    for i, name in enumerate(names):
+        t = arrays[name]
+        a = t.detach().cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t)
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        share = budget // (len(names) - i)  # what is left, split evenly over the arrays still to come
+        if a.nbytes > share:
+            if a.ndim == 0 or share < a.nbytes // max(1, a.shape[0]) + 8:
+                raise SystemExit(f"bench.py --dump-outputs: {name} does not fit the {DUMP_MAX_BYTES >> 20} MB budget")
+            row_bytes = a.nbytes // a.shape[0]
+            n_keep = share // (row_bytes + 8)  # + 8 bytes per row for its float64 index
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], n_keep, replace=False)).astype(np.float64)
+            np.save(os.path.join(out_dir, name + "_sample_rows.npy"), rows)
+            a = a[rows.astype(np.int64)]
+            budget -= rows.nbytes
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+        budget -= a.nbytes
 
 
 def cpu_port_rate(n_rays: int, threads: int, keep=None):
@@ -219,8 +247,8 @@ def bounded_cpu_rays(max_rays: int, rate: float, seconds: float) -> int:
 
 
 def run_reference(args):
-    """--impl reference: the reference's CPU path (oracle port; /root/reference does not exist on
-    the GPU box) timed on host cores, same workload/metric, bounded sample per step (about 10 s of
+    """--impl reference: the reference's CPU path (oracle port: the reference checkout is not needed
+    on a GPU host) timed on host cores, same workload/metric, bounded sample per step (about 10 s of
     CPU work each, so that W + K steps end within a few minutes on any host)."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
@@ -253,7 +281,7 @@ def workload_config(n_gpus, engine):
             "rays_per_frame": W * H, "frames_per_step": n_gpus, "nominal_samples_per_ray": NOMINAL_PER_RAY,
             "mlp_evaluations_per_ray": EVALS_PER_RAY, "engine": engine,
             "parallelism": f"ray-sharded x{n_gpus}, one all-gather of image tiles per frame" if n_gpus > 1 else "single GPU",
-            "l2": "per-frame uniforms are 497 MB (> 126 MB L2) and every step reads fresh ones; no explicit flush"}
+            "l2": "per-frame uniforms are 497 MB (> 50 MB L2) and every step reads fresh ones; no explicit flush"}
 
 
 # --------------------------------------------------------------------------------------------------
@@ -323,7 +351,7 @@ def train_config(engine):
                         "NeDDF 8x256 + 4x256 tanhExp, seeded random-init weights, set_iter(k)",
             "rays_per_step": TRAIN_RAYS, "nominal_samples_per_ray": NOMINAL_PER_RAY,
             "mlp_evaluations_per_ray": EVALS_PER_RAY, "engine": engine, "parallelism": "single GPU",
-            "l2": "1.3e9 B of per-step activations (> 126 MB L2) are written and re-read every step; no explicit flush"}
+            "l2": "1.3e9 B of per-step activations (> 50 MB L2) are written and re-read every step; no explicit flush"}
 
 
 def run_train(args):
@@ -375,6 +403,8 @@ def run_train(args):
     resident = [tuple(x.to(dev) for x in b) for b in host]
     it = [0]
 
+    last = {}
+
     def one_step(uv, color, mask):
         render.set_iter(it[0])
         it[0] += 1
@@ -383,6 +413,7 @@ def run_train(args):
         opt.zero_grad(set_to_none=True)
         loss.backward()
         opt.step()
+        last["out"], last["loss"] = out, loss
         return loss
 
     def step_device(i):
@@ -411,6 +442,11 @@ def run_train(args):
     launches = L.lib().neddf_launch_count() - launches0
     clocks = sampler.stop()
     render.check_status()
+    if args.dump_outputs:  # the last timed step: its loss, render outputs and the parameters after its Adam step
+        arrays = {"loss": last["loss"].reshape(1)}
+        arrays.update({k: v for k, v in last["out"].items() if isinstance(v, torch.Tensor) and v.is_floating_point()})
+        arrays.update({"param." + k: v for k, v in render.state_dict().items() if v.is_floating_point()})
+        dump_outputs(args.dump_outputs, arrays)
     for i in range(2):
         step_e2e(i)
     ms_e2e = timed(step_e2e, args.steps)
@@ -421,7 +457,7 @@ def run_train(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = peaks.get("bf16_tflops_sustained", 1400.0)
+    peak = peaks.get("bf16_tflops_sustained", H100_FP16_TFLOPS)
     achieved = evals * 3 * F_FULL / (ms_step * 1e-3) / 1e12
     cpu = None
     if not args.no_cpu_baseline:
@@ -464,7 +500,12 @@ def main():
                     help="early ray termination threshold on the transmittance (BASELINE.json configs[4]; 0 = off = "
                          "the reference's behaviour, the default workload)")
     ap.add_argument("--segments", type=int, default=4, help="depth segments of the fine pass when --eps > 0")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy "
+                         "(float32 / float64, at most 64 MB in all)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes what the CUDA path computed; it does not apply to --impl reference")
     if args.warmup < 3:
         args.warmup = 3  # timing rules: W >= 3
     if args.workload == "train":
@@ -515,6 +556,8 @@ def main():
     dev_u = [(a.to(dev), b.to(dev)) for a, b in host_u]
     targets = ["color", "depth"]
 
+    last = {}
+
     def step_device():
         outs = []
         for f in range(n_frames):
@@ -525,6 +568,7 @@ def main():
                 outs.append(gather_tiles(packed, n_pix))
             else:
                 outs.append(flat)
+        last["outs"] = outs
         return outs
 
     def step_e2e():
@@ -580,6 +624,14 @@ def main():
     launches = L.lib().neddf_launch_count() - launches0
     clocks = sampler.stop() if rank == 0 else None
     render.check_status()
+    if args.dump_outputs and rank == 0:  # the last timed step: this rank's colour / depth of every frame
+        arrays = {}
+        for f, o in enumerate(last["outs"]):
+            if world > 1:
+                arrays[f"frame{f}.color_depth"] = o
+            else:
+                arrays[f"frame{f}.color"], arrays[f"frame{f}.depth"] = o["color"], o["depth"]
+        dump_outputs(args.dump_outputs, arrays)
     term = render.termination_stats()  # fine-pass evaluations of this rank inside the timed region
     if world > 1:
         tt = torch.tensor([term["executed"], term["nominal"]], device=dev, dtype=torch.int64)
@@ -604,24 +656,9 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = peaks.get("bf16_tflops_sustained", 1400.0)
-    peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if peaks else "fallback (B200_PROFILING.md sustained 1.4 PFLOP/s)"
-    # DRAM bytes per launch of the dominant kernel from the committed ncu --set full capture; only valid for the
-    # kernel source it was taken from (hash of field_tc.cu + tc_ptx.cuh) and the engine it profiled
-    traffic, traffic_note = None, None
-    try:
-        import hashlib
-        tj = json.load(open(os.path.join(ROOT, "profiles", "field_kernel_traffic.json")))
-        h = hashlib.sha256(b"".join(open(os.path.join(ROOT, f), "rb").read() for f in tj["source_files"])).hexdigest()
-        if h != tj["source_sha256"]:
-            traffic_note = "profiles/field_kernel_traffic.json was captured from a different kernel source - re-run the ncu capture"
-        elif render.network_fine.resolved_engine(dev) != "tc":
-            traffic_note = "the committed capture is of the tc engine"
-        else:
-            traffic = tj["dram_bytes_per_launch"]
-            traffic_note = tj["launch"]
-    except Exception as e:  # noqa: BLE001
-        traffic_note = f"no capture available ({e})"
+    peak = peaks.get("bf16_tflops_sustained", H100_FP16_TFLOPS)
+    peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if peaks else "fallback (H100 SXM data sheet, dense FP16)"
+    traffic, traffic_note = None, "not measured (no DRAM-traffic capture of this kernel)"
 
     # end to end through the public API with host buffers
     for _ in range(2):

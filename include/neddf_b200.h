@@ -1,5 +1,5 @@
 /*
- * neddf_b200 -- C ABI of the B200-native NeDDF volumetric-rendering hot path.
+ * neddf_b200 -- C ABI of the H100-native (sm_90a) NeDDF volumetric-rendering hot path.
  *
  * This is the drop-in boundary: plain pointers and sizes, no torch types.  The reference
  * (ueda0319/neddf @ f71838ea) is pure Python/PyTorch and has no FFI of its own, so every
@@ -51,8 +51,8 @@ extern "C" {
 /* field engines */
 #define NEDDF_ENGINE_AUTO 0  /* TC when the configuration allows, else TC2, else fp32 */
 #define NEDDF_ENGINE_FP32 1  /* CUDA-core fp32 FMA megakernel (bit-faithful fp32 arithmetic) */
-#define NEDDF_ENGINE_TC 2    /* tcgen05 megakernel, 3-product fp16-split operands, fp32 accumulate; one CTA per SM */
-#define NEDDF_ENGINE_TC2 3   /* same arithmetic, CTA pairs (tcgen05 cta_group::2): half the weight stream per sample */
+#define NEDDF_ENGINE_TC 2    /* wgmma megakernel, 3-product fp16-split operands, fp32 accumulate; one CTA per SM */
+#define NEDDF_ENGINE_TC2 3   /* same kernel in 2-CTA clusters sharing the weight stream (TMA multicast): half the L2 reads per sample */
 
 /* output-selection flags for neddf_field_forward* */
 #define NEDDF_OUT_FULL 0      /* everything NeDDF.forward returns, incl. fields_penalty */
@@ -101,8 +101,8 @@ const char* neddf_last_error(void);
 int32_t neddf_field_layer_shapes(const neddf_field_config_t* cfg, int32_t* shapes_out, int32_t max_layers);
 
 /* NeDDF.__init__ (neddf.py:52-160): validates the configuration, allocates packed-weight
- * storage on the current device.  A handle also owns per-launch scratch of its kernels (status word, the parked
- * rows of the batched colour trunk, head partial sums of the pair kernel): launches on ONE handle must be
+ * storage on the current device.  A handle also owns per-launch scratch of its kernels (the status word):
+ * launches on ONE handle must be
  * stream-ordered with respect to each other (the reference's module is not re-entrant either); different
  * handles - e.g. the coarse and the fine network - are independent. */
 int32_t neddf_field_create(const neddf_field_config_t* cfg, neddf_field_t** out);
@@ -116,11 +116,6 @@ int32_t neddf_field_resolve_engine(const neddf_field_t* f, int32_t engine);
  * tensor-core engine met an activation outside fp16 range (|x| > 65504); results of that call are
  * invalid and the caller should use NEDDF_ENGINE_FP32 for this network. */
 int32_t neddf_field_status(const neddf_field_t* f, int32_t* h_status_out, void* stream);
-
-/* Profiling aid for the tensor-core engine: when d_buf != NULL, CTA 0 of every following launch
- * writes 4 SM-clock stamps per (tile, step) into d_buf[capacity] (int64): MMA phase start, MMA
- * issue done, epilogue start, epilogue done.  Pass NULL to switch it off. */
-int32_t neddf_field_set_timeline(neddf_field_t* f, int64_t* d_buf, int32_t capacity);
 
 /* The reference's training objective in one launch (loss/base_loss.py:45-85, color_loss.py:41-55,
  * mask_bce_loss.py:41-59, fields_constraint_loss.py:40-54; summed as nerf_trainer.py:118-121):
@@ -174,12 +169,6 @@ int32_t neddf_terminate_rays(const float* d_dists, const float* d_density, int64
                              int32_t edge0, int32_t seg_len, const int32_t* d_idx_in, const int32_t* d_n_in,
                              float* d_transmittance, float eps, int32_t* d_idx_out, int32_t* d_n_out,
                              uint64_t* d_executed, void* stream);
-
-/* Debugging aid for the tensor-core pair engine: when d_buf != NULL, cluster 0 of every following
- * launch copies, at (its first tile, hidden step `step`), per CTA the AUX operand buffer (hi parts,
- * 6144 words) and both accumulator halves (2 x 128 lanes x 128 columns fp32) into
- * d_buf[2][6144 + 32768].  Pass NULL to switch it off. */
-int32_t neddf_field_set_debug_dump(neddf_field_t* f, float* d_buf, int32_t step);
 
 /* Re-pack the module's parameters into kernel layout.  d_weights[i] is the i-th layer's
  * weight, fp32 [in,out] row-major exactly as LinearGradLayer stores it
@@ -319,40 +308,10 @@ int32_t neddf_invert_cdf(const float* d_dists, const float* d_cdf, const float* 
 /* How many kernels this library has launched since load (bench.py "gpu_launches"). */
 int64_t neddf_launch_count(void);
 
-/* Self-test of the tcgen05 GEMM building block: C[M,N] = A[M,K] * B[N,K]^T with fp16-split
- * operands; returns 0 and fills d_c.  Used by tests to pin the UMMA descriptor layouts. */
+/* Self-test of the wgmma GEMM building block: C[M,N] = A[M,K] * B[N,K]^T with fp16-split
+ * operands; returns 0 and fills d_c.  Used by tests to pin the descriptor layouts. */
 int32_t neddf_tc_selftest(const float* d_a, const float* d_b, int32_t m, int32_t n, int32_t k,
                           float* d_c, void* stream);
-
-/* Self-test of the "A operand in tensor memory" MMA form (weights written to TMEM with
- * tcgen05.st, activations MN-major in shared memory): C[128,128] = A[128,k] B[128,k]^T, averaged
- * over `reps` repeated accumulations; d_cycles[0] (optional) = SM cycles for reps*k/16*3 MMAs. */
-int32_t neddf_tc_selftest_ts(const float* d_a, const float* d_b, int32_t k, float* d_c, int64_t* d_cycles,
-                             int32_t reps, void* stream);
-
-/* tcgen05 issue-rate microbenchmark (profiling aid): reps x 16 MMAs 128 x n x 16 on resident
- * shared-memory operands; a_mn / b_mn = 1 for MN-major operands, swizzle 0 (none) or 2 (128B).
- * d_cycles[0] = SM cycles to issue, d_cycles[1] = cycles until the last MMA completed. */
-int32_t neddf_tc_mma_bench(int32_t a_mn, int32_t b_mn, int32_t swizzle, int32_t n, int32_t reps,
-                           int64_t* d_cycles, void* stream);
-
-/* Self-test of the CTA-pair MMA (tcgen05.mma.cta_group::2, cluster of two CTAs on one TPC):
- * C[256,n] = A[256,k] B[n,k]^T with A written to tensor memory by each CTA (rows 128r..128r+127) and
- * B MN-major in shared memory (CTA r holds rows (n/2)r..(n/2)(r+1)-1); averaged over `reps`
- * accumulations; d_cycles[0] (optional) = SM cycles for reps*k/16*3 MMAs.  Pins the operand split,
- * the multicast commit and the accumulator layout the pair kernel (field_tc2.cu) relies on. */
-int32_t neddf_tc_pair_selftest(const float* d_a, const float* d_b, int32_t n, int32_t k, float* d_c,
-                               int64_t* d_cycles, int32_t reps, void* stream);
-
-/* Distributed-shared-memory store rate (profiling aid): every CTA of n_clusters CTA pairs writes
- * `bytes` x reps with 16-byte st.shared::cluster (mode 0 = own shared memory, 1 = both CTAs into the
- * peer, 2 = rank 0 into rank 1 only, 3 = like 1 with 512-byte blocks permuted).  d_cycles[cta]. */
-int32_t neddf_dsmem_bench(int32_t mode, int32_t reps, int32_t bytes, int32_t n_clusters, int64_t* d_cycles,
-                          void* stream);
-
-/* tcgen05.cp layout probe (profiling / bring-up aid): one 128x256b shared-memory -> tensor-memory copy of
- * the 16-bit pattern value[i] = i with descriptor strides (lbo, sbo); d_out[128 lanes][8 columns]. */
-int32_t neddf_tc_cp_probe(int32_t lbo, int32_t sbo, uint32_t* d_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * NeRF field variant (SURVEY 8(f) item 3; neddf/network/nerf.py).  Forward only, fp32 CUDA-core kernel

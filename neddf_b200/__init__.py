@@ -1,4 +1,4 @@
-"""neddf_b200: B200-native (sm_100a) implementation of the NeDDF volumetric-rendering hot path
+"""neddf_b200: H100-native (sm_90a) implementation of the NeDDF volumetric-rendering hot path
 behind the reference's NeRFRender / NeDDF Python API.  See DESIGN.md."""
 from .camera import Camera, PinholeCalib  # noqa: F401
 from .network import BaseNeuralField, LinearGradLayer, NeDDF  # noqa: F401

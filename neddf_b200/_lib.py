@@ -1,7 +1,7 @@
 """ctypes binding of libneddf_b200.so (the C ABI declared in include/neddf_b200.h).
 
 There is no CPU or PyTorch fallback: if the shared library is missing or a call fails, the
-product raises.  Build it with ``python __graft_entry__.py`` (nvcc, sm_100a).
+product raises.  Build it with ``python __graft_entry__.py`` (nvcc, sm_90a).
 """
 import ctypes as C
 import os
@@ -9,7 +9,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# NEDDF_B200_LIB selects another build of the same ABI (tuning variants, tools/build_variant.py)
+# NEDDF_B200_LIB selects another build of the same ABI (e.g. a tuning variant)
 LIB_PATH = os.environ.get("NEDDF_B200_LIB") or os.path.join(_HERE, "libneddf_b200.so")
 
 MAX_SKIPS = 8
@@ -68,8 +68,6 @@ _SIGNATURES = {
     "neddf_field_create": (_I32, [C.POINTER(FieldConfig), C.POINTER(_P)]),
     "neddf_field_destroy": (_I32, [_P]),
     "neddf_field_resolve_engine": (_I32, [_P, _I32]),
-    "neddf_field_set_timeline": (_I32, [_P, _P, _I32]),
-    "neddf_field_set_debug_dump": (_I32, [_P, _P, _I32]),
     "neddf_field_status": (_I32, [_P, C.POINTER(C.c_int32), _P]),
     "neddf_field_set_weights": (_I32, [_P, C.POINTER(_P), C.POINTER(_P), _I32, _P]),
     "neddf_make_rays": (_I32, [_P, _I32, _I64, _FP, _FP, _FP, _P, _P, _P]),
@@ -100,12 +98,7 @@ _SIGNATURES = {
     "neddf_composite_backward": (_I32, [_P, _P, _P, _I64, _I32, _F, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "neddf_sample_pdf": (_I32, [_P, _P, _P, _I64, _I32, _I32, _I32, _P, _P, _P, _P, _P]),
     "neddf_invert_cdf": (_I32, [_P, _P, _P, _I64, _I32, _I32, _P, _P, _P]),
-    "neddf_tc_mma_bench": (_I32, [_I32, _I32, _I32, _I32, _I32, _P, _P]),
-    "neddf_tc_selftest_ts": (_I32, [_P, _P, _I32, _P, _P, _I32, _P]),
     "neddf_tc_selftest": (_I32, [_P, _P, _I32, _I32, _I32, _P, _P]),
-    "neddf_tc_pair_selftest": (_I32, [_P, _P, _I32, _I32, _P, _P, _I32, _P]),
-    "neddf_tc_cp_probe": (_I32, [_I32, _I32, _P, _P]),
-    "neddf_dsmem_bench": (_I32, [_I32, _I32, _I32, _I32, _P, _P]),
     "neddf_nerf_layer_shapes": (_I32, [C.POINTER(NerfConfig), C.POINTER(C.c_int32), _I32]),
     "neddf_nerf_create": (_I32, [C.POINTER(NerfConfig), C.POINTER(_P)]),
     "neddf_nerf_destroy": (None, [_P]),
@@ -139,7 +132,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"neddf_b200: {LIB_PATH} is missing - build it with `python __graft_entry__.py` "
-                "(nvcc, sm_100a). There is no CPU / PyTorch fallback for the render hot path.")
+                "(nvcc, sm_90a). There is no CPU / PyTorch fallback for the render hot path.")
         handle = C.CDLL(LIB_PATH)
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(handle, name)  # AttributeError if the ABI lost a symbol

@@ -226,57 +226,37 @@ extern "C" int32_t neddf_field_create(const neddf_field_config_t* cfg, neddf_fie
   return NEDDF_OK;
 }
 
-// AUTO: the single-CTA tensor-core kernel where it applies (the faster of the two today:
-// profiles/r02_summary.md), else the CTA-pair kernel (wider configuration coverage: any embedding ranks
-// that fit the 64 / 96 K of AUX), else fp32 FMA.  NEDDF_AUTO_ENGINE=tc2 flips the preference.
+// AUTO: the single-CTA tensor-core kernel where the tensor-core engines apply, else fp32 FMA.
+// NEDDF_AUTO_ENGINE=tc2 selects the CTA-pair form of the same kernel instead.
 static int32_t auto_engine(const neddf_field* f) {
   static const bool prefer_pair = [] {
     const char* e = std::getenv("NEDDF_AUTO_ENGINE");
     return e && std::string(e) == "tc2";
   }();
-  if (prefer_pair && tc2_supported(f)) return NEDDF_ENGINE_TC2;
-  if (tc_supported(f)) return NEDDF_ENGINE_TC;
-  if (tc2_supported(f)) return NEDDF_ENGINE_TC2;
-  return NEDDF_ENGINE_FP32;
+  if (!tc_supported(f)) return NEDDF_ENGINE_FP32;
+  return prefer_pair ? NEDDF_ENGINE_TC2 : NEDDF_ENGINE_TC;
 }
 
 extern "C" int32_t neddf_field_resolve_engine(const neddf_field_t* f, int32_t engine) {
   if (!f) return fail(NEDDF_E_INVALID, "neddf_field_resolve_engine: field is NULL");
   if (engine == NEDDF_ENGINE_AUTO) return auto_engine(f);
   if (engine == NEDDF_ENGINE_TC && !tc_supported(f)) return fail(NEDDF_E_UNSUPPORTED, "tensor-core engine does not cover this configuration");
-  if (engine == NEDDF_ENGINE_TC2 && !tc2_supported(f)) return fail(NEDDF_E_UNSUPPORTED, "tensor-core pair engine does not cover this configuration");
+  if (engine == NEDDF_ENGINE_TC2 && !tc_supported(f)) return fail(NEDDF_E_UNSUPPORTED, "tensor-core pair engine does not cover this configuration");
   if (engine != NEDDF_ENGINE_FP32 && engine != NEDDF_ENGINE_TC && engine != NEDDF_ENGINE_TC2) return fail(NEDDF_E_INVALID, "unknown engine id");
   return engine;
 }
 
-extern "C" int32_t neddf_field_set_timeline(neddf_field_t* f, int64_t* d_buf, int32_t capacity) {
-  if (!f) return fail(NEDDF_E_INVALID, "neddf_field_set_timeline: field is NULL");
-  if (!tc_supported(f) && !tc2_supported(f)) return fail(NEDDF_E_UNSUPPORTED, "timeline is a tensor-core engine facility");
-  int32_t rc = NEDDF_OK;
-  if (tc_supported(f)) rc = tc_set_timeline(f, reinterpret_cast<long long*>(d_buf), capacity);
-  if (rc == NEDDF_OK && tc2_supported(f)) rc = tc2_set_timeline(f, reinterpret_cast<long long*>(d_buf), capacity);
-  return rc;
-}
-
-extern "C" int32_t neddf_field_set_debug_dump(neddf_field_t* f, float* d_buf, int32_t step) {
-  if (!f) return fail(NEDDF_E_INVALID, "neddf_field_set_debug_dump: field is NULL");
-  if (!tc2_supported(f)) return fail(NEDDF_E_UNSUPPORTED, "the debug dump is a facility of the tensor-core pair engine");
-  return tc2_set_dump(f, d_buf, step);
-}
-
 extern "C" int32_t neddf_field_status(const neddf_field_t* f, int32_t* h_status_out, void* stream) {
   if (!f || !h_status_out) return fail(NEDDF_E_INVALID, "neddf_field_status: NULL argument");
-  int v = 0, v2 = 0;
+  int v = 0;
   int32_t rc = tc_read_status(f, &v, (cudaStream_t)stream);
-  if (rc == NEDDF_OK) rc = tc2_read_status(f, &v2, (cudaStream_t)stream);
-  *h_status_out = v | v2;
+  *h_status_out = v;
   return rc;
 }
 
 extern "C" int32_t neddf_field_destroy(neddf_field_t* f) {
   if (!f) return NEDDF_OK;
   tc_destroy(f);
-  tc2_destroy(f);
   cudaFree(f->d_w_hidden);
   cudaFree(f->d_b_hidden);
   cudaFree(f->d_w_head_da);
@@ -319,10 +299,6 @@ extern "C" int32_t neddf_field_set_weights(neddf_field_t* f, const float* const*
     int32_t rc = tc_pack_weights(f, d_weights, d_biases, s);
     if (rc != NEDDF_OK) return rc;
   }
-  if (tc2_supported(f)) {
-    int32_t rc = tc2_pack_weights(f, d_weights, d_biases, s);
-    if (rc != NEDDF_OK) return rc;
-  }
   {
     int32_t rc = pack_backward_weights(f, d_weights, s);
     if (rc != NEDDF_OK) return rc;
@@ -353,12 +329,12 @@ static int32_t fill_state(const neddf_field* f, const neddf_field_state_t* st, F
 static int32_t dispatch(const neddf_field* f, FieldParams& p, int32_t flags, int32_t engine, cudaStream_t s) {
   if (engine == NEDDF_ENGINE_AUTO) engine = auto_engine(f);
   if (engine == NEDDF_ENGINE_TC2) {
-    if (!tc2_supported(f)) return fail(NEDDF_E_UNSUPPORTED, "tensor-core pair engine does not cover this configuration");
-    return launch_field_tc2(f, p, flags, s);
+    if (!tc_supported(f)) return fail(NEDDF_E_UNSUPPORTED, "tensor-core pair engine does not cover this configuration");
+    return launch_field_tc(f, p, flags, true, s);
   }
   if (engine == NEDDF_ENGINE_TC) {
     if (!tc_supported(f)) return fail(NEDDF_E_UNSUPPORTED, "tensor-core engine does not cover this configuration");
-    return launch_field_tc(f, p, flags, s);
+    return launch_field_tc(f, p, flags, false, s);
   }
   if (engine == NEDDF_ENGINE_FP32) return launch_field_fp32(f, p, s);
   return fail(NEDDF_E_INVALID, "unknown engine id");

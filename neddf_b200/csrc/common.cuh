@@ -1,4 +1,4 @@
-// Shared helpers for the neddf_b200 kernels (sm_100a only).
+// Shared helpers for the neddf_b200 kernels (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -41,7 +41,7 @@ inline int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;  // H100 SXM
   }
   return n;
 }

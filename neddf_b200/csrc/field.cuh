@@ -121,9 +121,8 @@ struct neddf_field {
   float* d_wt_hidden = nullptr;  // backward: transposed h-part of every hidden layer l >= 1, packed like w_hidden
   int wt_chunks = 0;
   bool weights_set = false;
-  // tensor-core engine storage (field_tc.cu) and its CTA-pair variant (field_tc2.cu)
+  // tensor-core engine storage (field_tc.cu), shared by "tc" and "tc2"
   void* tc = nullptr;
-  void* tc2 = nullptr;
 };
 
 namespace neddf {
@@ -132,17 +131,9 @@ int32_t launch_field_backward(const neddf_field* f, FieldParams& p, const Backwa
 int32_t pack_backward_weights(neddf_field* f, const float* const* d_w, cudaStream_t s);
 
 int32_t tc_pack_weights(neddf_field* f, const float* const* d_w, const float* const* d_b, cudaStream_t s);
-int32_t launch_field_tc(const neddf_field* f, FieldParams& p, int flags, cudaStream_t s);
-bool tc_supported(const neddf_field* f);
+// pair = engine "tc2": the same kernel in clusters of two CTAs sharing the weight stream
+int32_t launch_field_tc(const neddf_field* f, FieldParams& p, int flags, bool pair, cudaStream_t s);
+bool tc_supported(const neddf_field* f);  // engines "tc" and "tc2"
 void tc_destroy(neddf_field* f);
-int32_t tc_set_timeline(neddf_field* f, long long* d_buf, int cap);
 int32_t tc_read_status(const neddf_field* f, int* out, cudaStream_t s);
-
-int32_t tc2_pack_weights(neddf_field* f, const float* const* d_w, const float* const* d_b, cudaStream_t s);
-int32_t launch_field_tc2(const neddf_field* f, FieldParams& p, int flags, cudaStream_t s);
-bool tc2_supported(const neddf_field* f);
-void tc2_destroy(neddf_field* f);
-int32_t tc2_set_timeline(neddf_field* f, long long* d_buf, int cap);
-int32_t tc2_read_status(const neddf_field* f, int* out, cudaStream_t s);
-int32_t tc2_set_dump(neddf_field* f, float* d_buf, int step);
 }  // namespace neddf

@@ -4,7 +4,7 @@
 // get_sampling_points (neddf/ray/ray.py:88-194) optionally fused into the prologue.
 //
 // This engine does every multiply-add in fp32 FMA, so it is the bit-faithful device
-// statement of the network and the in-repo device oracle for the tcgen05 engine.
+// statement of the network and the in-repo device oracle for the tensor-core engines.
 //
 // Work decomposition
 //   CTA (256 threads) = one tile of 16 samples; grid = #SMs, persistent over tiles.

@@ -1,12 +1,12 @@
-// K2 (tensor-core engine): the NeDDF field network as one persistent tcgen05 megakernel.
+// K2 (tensor-core engines "tc" and "tc2"): the NeDDF field network as one persistent wgmma megakernel (sm_90a).
 //
 // Reference: NeDDF.forward (neddf/network/neddf.py:162-309), sample geometry of
 // neddf/ray/ray.py:88-194 fused into the prologue.
 //
 // Precision.  Parity with the fp32 reference (1e-4) rules out single-pass TF32/BF16/FP16 operands
 // (measured 1e-3..1e-2, SURVEY 7.3).  Every GEMM operand is therefore split x = hi + lo into two
-// fp16 values and three products are accumulated in fp32 in TMEM:
-//     hi_w*hi_x + lo_w*hi_x + hi_w*lo_x        (kind::f16, fp32 accumulate)
+// fp16 values and three products are accumulated in fp32:
+//     hi_w*hi_x + lo_w*hi_x + hi_w*lo_x        (wgmma f16, fp32 accumulate)
 // which is as accurate as 3xTF32 (emulated on the oracle: density 3.5e-6, colour 1.7e-6) at twice
 // TF32's tensor rate.  fp16's range (65504) is checked in the epilogue; a tile that exceeds it sets
 // status bit 2 and the host raises (the fp32 engine covers such networks).
@@ -15,128 +15,113 @@
 // d/dy, d/dz), so the value rows are the first 32 rows of every operand: when only images are
 // wanted (no fields_penalty) the colour trunk runs on N = 32 rows instead of 128.
 //
-// Orientation.  Every sample carries 4 rows (value + d/dx, d/dy, d/dz).  The MMAs are issued
-// "swapped": A = weights (M = 128 output channels), B = activations (N = 128 rows = 32 samples x 4,
-// MN-major in shared memory), so the accumulator has one output channel per TMEM lane and the rows
-// of a sample in columns.  The epilogue thread that owns a channel therefore holds x and its three
-// Jacobian entries in registers: y = f(x), G = f'(x) J need no cross-thread traffic, and it writes
-// 8 consecutive rows (16 bytes) of the next layer's B operand per store.  The narrow heads
-// (256->1,1,3) run in the standard orientation (A = activations, N = 16) so that their result has
-// one sample row per lane.
+// Orientation.  The MMAs are issued "swapped": A = weights (M = output channels, K-major), B =
+// activations (N = 128 rows = 32 samples x 4, MN-major in shared memory), so a thread's accumulator
+// fragment holds, for each of its channels, x and the three Jacobian entries of the same samples:
+// y = f(x), G = f'(x) J need no cross-thread traffic, and the epilogue writes the next layer's B
+// operand straight from registers.  The narrow heads (256 -> 1, 1, 3) are dot products over the
+// 256 channels in fp32 (hi + lo of the operand), 8 threads per sample.
 //
-// A operand in tensor memory.  With A in shared memory a 128xNx16 tcgen05.mma costs ~133 cycles for
-// any N <= 256 (the A fetch sets the rate, tools/mma_bench.py); with A in tensor memory it costs
-// the 64-cycle floor (tools/ts_test.py).  The weights therefore never enter shared memory: loader
-// warps read each 8 KB chunk from L2 (LDG.128, prefetched in registers) and write it into a
-// 16-stage ring of TMEM columns with tcgen05.st.
-//
-// Per SM: one CTA of 25 warps, persistent over 32-sample tiles.
-//   warps 0-15  epilogue: TMEM -> registers (tcgen05.ld), bias + activation + Jacobian, fp16
-//               hi/lo split, st.shared into the next B operand; also prologue (geometry, PE).
-//               warp w: TMEM lane quarter w%4, channel half (w/4)%2 (= epilogue group), sample
-//               half w/8
-//   warp  16    MMA issuer: convergent warp, one elected lane issues tcgen05.mma / tcgen05.commit
-//   warps 17-24 weight loaders: L2 -> registers -> tensor memory, two warps per lane quarter
+// Per CTA: 288 threads, persistent over 32-sample tiles.
+//   warpgroups 0, 1   consumers: warpgroup g owns output channels [128g, 128g + 128) (two m64 blocks,
+//                     128 fp32 accumulators per thread); prologue, epilogues and heads
+//   warp 8            producer: one lane streams the weight chunks (16 K x 256 channels, fp16 hi | lo,
+//                     16 KB) from L2 into a 3-stage shared-memory ring with TMA bulk copies
 // Shared memory (B operands, canonical no-swizzle MN-major: [row/8][k][row%8] fp16):
 //   H   hi/lo  128 rows x 256 k   2 x 64 KB   hidden activations, rewritten layer after layer
 //   AUX hi/lo  128 rows x  96 k   2 x 24 KB   E_s (trunk input + skip) then [E0|D|n] (colour input)
-//   head weights 4 x 8 KB (resident)
-// TMEM (512 columns): accumulator of channel half h at [128h, 128h+128); head results alias
-// columns [0,16); weight ring at [256, 512), 16 columns (8 hi + 8 lo) per chunk.
+//   ring       3 x 16 KB                      weight chunks
+//
+// "tc2" runs the same program in clusters of two CTAs: each CTA fetches half of every weight chunk and
+// multicasts it into both CTAs' rings, which halves the L2 -> SM weight traffic per tile.  The two CTAs
+// of a cluster consume the chunk stream in lockstep (a CTA whose partner has one tile more runs an empty
+// tile); a ring stage is refilled once the consumers of both CTAs have released it.
 #include "tc_ptx.cuh"
 
 #include <algorithm>
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
-#include <type_traits>
 
 namespace neddf {
 namespace tc {
 
-constexpr int kStageBytes = kChunkBytes;
-constexpr int kARing = 16;          // weight chunks resident in tensor memory (16 columns each)
-constexpr int kEpiWarps = 16;
-constexpr int kEpiThreads = kEpiWarps * 32;
-constexpr int kMmaWarp = kEpiWarps;          // warp 16
-#ifndef NEDDF_TC_LOAD_WARPS
-#define NEDDF_TC_LOAD_WARPS 8   // tuning knobs for experiments (tools/build_variant.py); the shipped values
-#endif
-#ifndef NEDDF_TC_LOAD_DEPTH
-#define NEDDF_TC_LOAD_DEPTH 3   // are the measured best (profiles/r01_summary.md)
-#endif
-constexpr int kLoadWarps = NEDDF_TC_LOAD_WARPS;               // warps 17-24: lane quarter w%4, chunk parity (w-17)/4
-constexpr int kLoadPerQuarter = kLoadWarps / 4;  // loader warps per TMEM lane quarter, taking chunks round-robin
-constexpr int kThreads = kEpiThreads + 32 + kLoadWarps * 32;
-constexpr uint32_t kACol = 256;              // first TMEM column of the weight ring
-constexpr int kMaxSteps = kMaxHidden + 2;
-constexpr uint32_t kTmemCols = 512;
-constexpr uint32_t kHeadCol = 0;  // head results alias the (then idle) hidden accumulators
+constexpr int kStages = 3;
+constexpr int kConsumers = 256;                 // two warpgroups
+constexpr int kConsumerWarps = kConsumers / 32;
+constexpr int kThreads = kConsumers + 32;       // + the producer warp
 
 constexpr uint32_t kOffHHi = 0;
 constexpr uint32_t kOffHLo = kOffHHi + kHBytes;
 constexpr uint32_t kOffAuxHi = kOffHLo + kHBytes;
 constexpr uint32_t kOffAuxLo = kOffAuxHi + kAuxBytes;
-constexpr uint32_t kOffHeadW = kOffAuxLo + kAuxBytes;       // (ddf,aux) hi | lo | colour hi | lo
-constexpr uint32_t kOffScratch = kOffHeadW + 4 * kChunkBytes;
+constexpr uint32_t kOffRing = kOffAuxLo + kAuxBytes;
+constexpr uint32_t kOffScratch = kOffRing + kStages * kChunkBytes;
 
 struct Scratch {
-  float geo[2][kTileS][12];   // pos[3], dir[3], var[3], pad; two buffers: the batched program fetches the next tile's early
-  HeadOut head[kTileS];
-  float hgather[4][kTileS][4];  // head results per row type (lane quarter) and sample
-  uint64_t a_full[kARing];   // loaders -> MMA: chunk written to tensor memory
-  uint64_t a_empty[kARing];  // MMA -> loaders: chunk consumed
-  uint64_t act_ready[2];  // epilogue group h -> MMA: accumulator h drained, H[k-half h] rewritten
-  uint64_t acc_ready[2];  // MMA -> epilogue group h: accumulator h complete
-  uint64_t stash_bar;     // bulk copies stash -> H / AUX landed (batched colour trunk)
-  uint32_t tmem_base;
-  uint32_t pad;
+  float geo[kTileS][12];     // pos[3], dir[3], var[3], pad
+  uint64_t full[kStages];    // producer(s) -> consumers: chunk landed
+  uint64_t empty[kStages];   // consumer warps (of both CTAs of a pair) -> producer: stage free
 };
 constexpr uint32_t kSmemBytes = kOffScratch + sizeof(Scratch);
 static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
 
-enum StepKind { kStepHidden = 0, kStepHeadDA = 1, kStepHeadCol = 2 };
-
-struct Step {
-  int kind;
+struct TcLayer {
   int aux_ksteps;  // K-steps (16) taken from AUX first ...
   int h_ksteps;    // ... then from H
-  int bias_off;    // hidden layers: offset into the plain-order bias array
-  int post;        // work the epilogue warps do after this step's epilogue, overlapping the next
-                   // step's MMA phase: 1 = colour-trunk inputs E0|D into AUX, 2 = next tile's prologue
 };
 
 struct TcParams {
   FieldParams f;
-  int n_steps;
+  TcLayer layer[kMaxHidden];
   int chunks_per_tile;
-  Step step[kMaxSteps];
-  const unsigned char* w_tc;  // packed chunks, kStageBytes each, in consumption order
+  const unsigned char* w_tc;  // packed chunks, kChunkBytes each, in consumption order
   const float* bias;          // [n_hidden][256] plain channel order
   int* status;
-  int head_da_step;     // index of the distance/aux heads step
-  int eval;             // 1 = images only: colour trunk on value rows (N = 32), no penalty / colour Jacobian
-  int debug;            // profiling aid (NEDDF_TC_DEBUG): 1 = skip the MMAs, 2 = loaders skip the L2 reads,
-                        // 4 = loaders skip the TMEM stores, 8 = epilogue skips the hidden-layer math; results are garbage
-  long long* timeline;  // optional: CTA 0 writes 6 values per step (profiling aid)
-  int timeline_cap;
-  // Batched colour trunk (images only): `batch` tiles run the distance trunk one after the other, park the value
-  // rows of their features and colour inputs in `stash`, then ONE pass of the colour trunk serves all of them as
-  // the 128 rows of the operand (row = 32 slot + sample): the colour weights are streamed once per 128 samples
-  // and its MMAs are N = 128 instead of N = 32.  batch == 1 is the per-tile program.
-  int batch;
-  int n_trunk;        // steps of the distance trunk incl. its heads (= head_da_step + 1)
-  int chunks_trunk;   // weight chunks of those steps (the colour trunk's follow in the packed stream)
-  unsigned char* stash;  // [CTA][slot][H hi 16 KB | H lo 16 KB | AUX hi 6 KB | AUX lo 6 KB] value rows in operand layout
+  int eval;                   // 1 = images only: colour trunk on value rows (N = 32), no penalty / colour Jacobian
 };
-constexpr uint32_t kStashH = 4 * kHK * 16;      // four row groups (32 value rows) of H: 16 KB
-constexpr uint32_t kStashAux = 4 * kAuxK * 16;  // of AUX: 6 KB
-constexpr uint32_t kStashSlot = 2 * kStashH + 2 * kStashAux;
-constexpr int kMaxBatch = kRows / kTileS;       // 4 slots
-constexpr uint32_t kStashCta = kMaxBatch * kStashSlot;
 
 // ---------------------------------------------------------------------------------------------
-// prologue pieces (epilogue warps)
+// cluster helpers (tc2)
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+__device__ __forceinline__ uint32_t mapa_u32(uint32_t saddr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
+  return r;
+}
+__device__ __forceinline__ void mbar_arrive_remote(uint32_t caddr) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(caddr) : "memory");
+}
+__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "TC_WAITC:\n"
+      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n"
+      "@p bra TC_DONEC;\n"
+      "bra TC_WAITC;\n"
+      "TC_DONEC:\n"
+      "}\n" ::"r"(smem_u32(bar)),
+      "r"(parity)
+      : "memory");
+}
+// bulk copy into the same shared-memory offset of both CTAs of the pair, completion on each CTA's mbarrier
+__device__ __forceinline__ void tma_bulk_g2s_pair(uint32_t dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(
+          dst_smem),
+      "l"(src), "r"(bytes), "r"(smem_u32(bar)), "h"((uint16_t)3)
+      : "memory");
+}
+
+// ---------------------------------------------------------------------------------------------
+// prologue pieces
 // ---------------------------------------------------------------------------------------------
 // geometry of the tile's samples -> scratch (one thread per sample)
 __device__ __forceinline__ void tile_geometry(const FieldParams& p, float (*geo)[12], int64_t n0, int s, int64_t n_total) {
@@ -183,18 +168,19 @@ __device__ __forceinline__ void write_pos_embedding(const FieldParams& p, const 
     PeEntry q = pe_entry(e, geo[s][d], geo[s][6 + d], p.lowpass[e]);
     float sc_ = scaled ? q.scale_s : q.scale_0;
     float g = q.freq * sc_;
-    // the Jacobian of entry (e, d) is non-zero in row type 1 + d only (selects, not an indexed local array: that
-    // array lived in local memory and the prologue was several thousand cycles of LDL / STL round trips)
+    // the Jacobian of entry (e, d) is non-zero in row type 1 + d only (selects, not an indexed local array)
     const float js = g * q.c, jc = -g * q.s;
     store_sample(aux_hi, aux_lo, kAuxK, s, idx, sc_ * q.s, d == 0 ? js : 0.f, d == 1 ? js : 0.f, d == 2 ? js : 0.f, bad, rows);
     store_sample(aux_hi, aux_lo, kAuxK, s, half + idx, sc_ * q.c, d == 0 ? jc : 0.f, d == 1 ? jc : 0.f, d == 2 ? jc : 0.f, bad, rows);
   }
 }
 
+__device__ __forceinline__ void bar_consumers() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory"); }
+
 // ---------------------------------------------------------------------------------------------
 // the megakernel
 // ---------------------------------------------------------------------------------------------
-template <int ACT>
+template <int ACT, bool PAIR>
 __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_constant__ TcParams P) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const FieldParams& p = P.f;
@@ -202,892 +188,403 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
   unsigned char* h_lo = smem + kOffHLo;
   unsigned char* aux_hi = smem + kOffAuxHi;
   unsigned char* aux_lo = smem + kOffAuxLo;
-  unsigned char* head_w = smem + kOffHeadW;
+  unsigned char* ring = smem + kOffRing;
   Scratch* sc = reinterpret_cast<Scratch*>(smem + kOffScratch);
 
   const int tid = threadIdx.x;
-  // Warp index, tile count and the tensor-memory base go through a shuffle so that ptxas can prove them
-  // warp-uniform: the MMA issuer's loop then runs on the uniform datapath (descriptors in uniform registers,
-  // three UTCHMMA back to back) instead of ~17 R2UR moves per chunk under an elected lane.
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-  const int lane = tid & 31;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int n_hidden = p.n_ddf + p.n_col;
 
+  // tiles: single CTAs take tiles blockIdx.x + t * gridDim.x; a pair takes tile pairs, CTA r the tile 2 pair + r
   const int64_t n_total = field_total(p);
   const int64_t n_tiles = (n_total + kTileS - 1) / kTileS;
+  const uint32_t rank = PAIR ? cluster_ctarank() : 0;
+  const int64_t unit = PAIR ? (int64_t)(blockIdx.x >> 1) : (int64_t)blockIdx.x;
+  const int64_t n_units = PAIR ? (int64_t)(gridDim.x >> 1) : (int64_t)gridDim.x;
+  const int64_t units_total = PAIR ? (n_tiles + 1) / 2 : n_tiles;
   int64_t my_tiles = 0;
-  if ((int64_t)blockIdx.x < n_tiles) my_tiles = (n_tiles - 1 - blockIdx.x) / gridDim.x + 1;
-  my_tiles = __shfl_sync(0xffffffffu, my_tiles, 0);
-  const int chunks_colour = P.chunks_per_tile - P.chunks_trunk;
-  const int64_t n_groups = (my_tiles + P.batch - 1) / P.batch;
-  const int64_t total_chunks = my_tiles * P.chunks_trunk + n_groups * chunks_colour;
+  if (unit < units_total) my_tiles = (units_total - 1 - unit) / n_units + 1;
+  auto tile_of = [&](int64_t t) { return PAIR ? 2 * (unit + t * n_units) + rank : unit + t * n_units; };
 
   if (tid == 0) {
-    for (int i = 0; i < kARing; ++i) {
-      mbar_init(&sc->a_full[i], 4);           // one arrival per lane quarter (4 loader warps per chunk)
-      mbar_init(&sc->a_empty[i], 1);          // tcgen05.commit
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&sc->full[i], 1);
+      mbar_init(&sc->empty[i], PAIR ? 2 * kConsumerWarps : kConsumerWarps);
     }
-    for (int h = 0; h < 2; ++h) {
-      mbar_init(&sc->act_ready[h], kEpiThreads / 2);
-      mbar_init(&sc->acc_ready[h], 1);
-    }
-    mbar_init(&sc->stash_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  // head weights (B operands of the standard-orientation head MMAs) stay resident: 4 x 8 KB
-  {
-    const uint4* src = reinterpret_cast<const uint4*>(P.w_tc + (size_t)P.chunks_per_tile * kChunkBytes);
-    uint4* dst = reinterpret_cast<uint4*>(head_w);
-    for (int i = tid; i < 4 * kChunkBytes / 16; i += kThreads) dst[i] = __ldg(src + i);
-  }
-  if (warp == kMmaWarp) tmem_alloc(&sc->tmem_base, kTmemCols);
-  fence_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = __shfl_sync(0xffffffffu, sc->tmem_base, 0);
+  if (PAIR) cluster_sync_all();  // the partner's barriers exist before any multicast or remote arrival
 
-  if (warp > kMmaWarp) {
-    // ===================== weight loaders: L2 -> registers -> tensor memory ======================
-    // Chunk (K-step, channel half) = 128 rows x [8 words hi | 8 words lo] (two fp16 per word).
-    // Lane = row of this warp's TMEM lane quarter; 64 contiguous bytes per lane, 2 KB per warp.
-    // Eight warps: two per lane quarter, taking alternate chunks, so that more loads are in
-    // flight than the L2 latency x 42 B/clk the tensor core consumes.
-    const int quarter = warp & 3;
-    const int cpar = (warp - kMmaWarp - 1) >> 2;  // this warp loads chunks g with (g & 1) == cpar
-    const uint32_t lane_addr = (uint32_t)(32 * quarter) << 16;
-    const uint4* base = reinterpret_cast<const uint4*>(P.w_tc) + (size_t)(32 * quarter + lane) * 4;
-    constexpr int kDepth = NEDDF_TC_LOAD_DEPTH;  // own chunks in flight in registers (= 6 chunks ahead of the MMA warp)
-    uint4 r[kDepth][4];
-    auto fetch = [&](int slot, int chunk) {
-      const uint4* src = base + (size_t)chunk * (kChunkBytes / 16);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) r[slot][j] = __ldg(src + j);
-    };
-    // Consumption order: per group of `batch` tiles the trunk chunks [0, chunks_trunk) once per tile, then the
-    // colour chunks [chunks_trunk, chunks_per_tile) once.  Both counts are even, so the index of chunk g within
-    // the packed stream has the parity of g.
-    // (32-bit counters: a CTA's share of a launch is far below 2^31 chunks, and the loader warps have no register to spare)
-    const int total = (int)total_chunks;
-    int fidx = cpar;  // index (in the packed stream) of the next chunk to fetch
-    int gf = cpar;
-    int f_ti = 0;                  // tile of the group being fetched
-    int f_left = (int)my_tiles;    // tiles not yet begun, incl. this group
-    int f_ng = f_left < P.batch ? f_left : P.batch;
-    auto advance = [&]() {
-      fidx += kLoadPerQuarter;
-      gf += kLoadPerQuarter;
-      if (f_ti < f_ng) {              // in the trunk stream of tile f_ti
-        if (fidx >= P.chunks_trunk) {
-          if (++f_ti < f_ng) fidx -= P.chunks_trunk;  // next tile of the group; else run on into the colour chunks
-        }
-      } else if (fidx >= P.chunks_per_tile) {  // colour stream done: next group
-        fidx -= P.chunks_per_tile;
-        f_left -= f_ng;
-        f_ng = f_left < P.batch ? f_left : P.batch;
-        f_ti = 0;
-      }
-    };
-#pragma unroll
-    for (int i = 0; i < kDepth; ++i) {
-      if (gf < total) {
-        fetch(i, fidx);
-        advance();
-      }
-    }
-    int stage = cpar;
-    uint32_t par = 0;
-    bool first_pass = true;
-    int g = cpar;
-    while (g < total) {
-#pragma unroll
-      for (int i = 0; i < kDepth; ++i) {
-        if (g < total) {
-          if (!first_pass) mbar_wait(&sc->a_empty[stage], par);
-          tc_fence_after();
-          const uint32_t ta = tmem + lane_addr + kACol + stage * 16;
-          const uint32_t w0[8] = {r[i][0].x, r[i][0].y, r[i][0].z, r[i][0].w, r[i][1].x, r[i][1].y, r[i][1].z, r[i][1].w};
-          const uint32_t w1[8] = {r[i][2].x, r[i][2].y, r[i][2].z, r[i][2].w, r[i][3].x, r[i][3].y, r[i][3].z, r[i][3].w};
-          if (!(P.debug & 4)) {
-            tmem_st16(ta, w0, w1);  // 8 hi words | 8 lo words of this lane's row
-          }
-          if (gf < total) {  // refill this register slot (the scoreboard orders it after the stores read it)
-            if (!(P.debug & 2)) fetch(i, fidx);
-            advance();
-          }
-          tmem_st_wait();
-          tc_fence_before();
-          if (lane == 0) mbar_arrive(&sc->a_full[stage]);
-          g += kLoadPerQuarter;
-          stage += kLoadPerQuarter;
-          if (stage >= kARing) {
-            stage -= kARing;
-            if (first_pass) first_pass = false;
-            else par ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    // ===================== MMA issuer (whole warp, one elected lane issues) ===================
-    const uint32_t s_hhi = smem_u32(h_hi), s_ahi = smem_u32(aux_hi), s_hlo = smem_u32(h_lo), s_alo = smem_u32(aux_lo);
-    const uint32_t s_head = smem_u32(head_w);
-    int stage = 0;          // ring position of the next chunk
-    uint32_t full_par = 0;  // parity to wait for on a_full[stage]
-    uint32_t act_phase = 0;
-    const bool batched = P.batch > 1;
-    int tl = 0;  // step instance counter (profiling stamps)
-    // program: per group of `batch` tiles the trunk steps [0, n_trunk) of every tile, then the colour steps once
-    for (int64_t t0 = 0; t0 < my_tiles; t0 += P.batch) {
-      const int ng = (int)((my_tiles - t0 < P.batch) ? my_tiles - t0 : P.batch);
-      for (int ti = 0; ti <= ng; ++ti) {  // ti == ng: the colour steps
-      const int si_begin = ti < ng ? 0 : P.n_trunk, si_end = ti < ng ? P.n_trunk : P.n_steps;
-      for (int si = si_begin; si < si_end; ++si, ++tl) {
-        const Step& st = P.step[si];
-        const bool stamp = P.timeline && blockIdx.x == 0 && lane == 0 && (tl + 1) * 6 <= P.timeline_cap;
-        // act_ready[h] of the previous step: epilogue group h has drained accumulator h and
-        // rewritten H[k-half h].  The first layer of a tile reads AUX written by both groups; so does the first
-        // colour layer (colour inputs / normals, or the parked rows that all threads bring back).
-        mbar_wait(&sc->act_ready[0], act_phase);
-        // (the heads start on K-half 0 as soon as group 0 has rewritten it and wait for group 1 half way)
-        if (si == 0 || si == P.n_trunk) mbar_wait(&sc->act_ready[1], act_phase);
-        tc_fence_after();
-        if (stamp) P.timeline[6 * tl + 0] = clock64();
-        if (st.kind == kStepHidden) {
-          // Per (K-step, channel half) one weight chunk in tensor memory and three MMAs
-          //   D_half += A_hi*B_hi + A_lo*B_hi + A_hi*B_lo          (A from TMEM: 64 cycles each)
-          // Issue order (half 0, G0), (half 1, G0), (half 0, G1), (half 1, G1) - see chunk_pos():
-          // half 0 completes a quarter layer early, so the two epilogue groups trail the tensor
-          // core instead of alternating with it.
-          const int nA = st.aux_ksteps, n1 = st.h_ksteps / 2, n0 = nA + st.h_ksteps - n1;
-          const uint64_t dba_hi = make_desc(s_ahi, 128, kAuxK * 16), dba_lo = make_desc(s_alo, 128, kAuxK * 16);
-          const uint64_t dbh_hi = make_desc(s_hhi, 128, kHK * 16), dbh_lo = make_desc(s_hlo, 128, kHK * 16);
-          // images only: the colour trunk (every hidden step after the distance heads) needs no
-          // Jacobian rows - the value rows are rows 0..31 of the same operands
-          const uint32_t idesc = (P.eval && si > P.head_da_step && !batched) ? kIdescHiddenValue : kIdescHidden;
-          // One asm block per chunk (a single elect, three MMAs, the commit that frees the ring
-          // stage) and no per-iteration selects: the issuing warp shares its scheduler with six other
-          // warps, and every instruction between two chunks is tensor-core idle time once the MMA
-          // queue runs dry (tools/timeline.py, debug modes).
-          auto run = [&](uint32_t d, uint64_t db_hi, uint64_t db_lo, int n, uint32_t& acc) {
-            for (int i = 0; i < n; ++i) {
-              mbar_wait(&sc->a_full[stage], full_par);
-              tc_fence_after();
-              chunk_mma_elect(d, tmem + kACol + stage * 16, db_hi, db_lo, idesc, acc, smem_u32(&sc->a_empty[stage]));
-              acc = 1;
-              db_hi += 16;  // 16 K = 256 bytes in descriptor units
-              db_lo += 16;
-              if (++stage == kARing) {
-                stage = 0;
-                full_par ^= 1;
-              }
-            }
-          };
-          auto issue = [&](int half, int ks_begin, int ks_end) {
-            const uint32_t d = tmem + half * kRows;
-            uint32_t acc = ks_begin > 0;
-            const int a_end = ks_end < nA ? ks_end : nA;
-            if (ks_begin < a_end) run(d, dba_hi + ks_begin * 16, dba_lo + ks_begin * 16, a_end - ks_begin, acc);
-            const int h_begin = ks_begin > nA ? ks_begin : nA;
-            if (h_begin < ks_end) run(d, dbh_hi + (h_begin - nA) * 16, dbh_lo + (h_begin - nA) * 16, ks_end - h_begin, acc);
-          };
-          issue(0, 0, n0);
-          if (si != 0 && si != P.n_trunk) {  // accumulator 1 free, H[k >= 128] ready
-            mbar_wait(&sc->act_ready[1], act_phase);
-            tc_fence_after();
-          }
-          issue(1, 0, n0);
-          issue(0, n0, n0 + n1);
-          mma_commit_elect(&sc->acc_ready[0]);
-          issue(1, n0, n0 + n1);
-          mma_commit_elect(&sc->acc_ready[1]);
-        } else {
-          // heads (standard orientation): D[row, n] = sum_k H[row,k] * Wh[n,k], weights resident
-          const uint32_t w = s_head + (st.kind == kStepHeadDA ? 0 : 2 * kChunkBytes);
-          const uint32_t d = tmem + kHeadCol;
-          uint64_t da_hi = make_desc(s_hhi, 128, kHK * 16), da_lo = make_desc(s_hlo, 128, kHK * 16);
-          uint64_t db_hi = make_desc(w, 128, 4096), db_lo = make_desc(w + kChunkBytes, 128, 4096);
-          for (int ks = 0; ks < kHK / 16; ++ks) {
-            if (ks == kHK / 32) {  // H[k >= 128] is group 1's
-              mbar_wait(&sc->act_ready[1], act_phase);
-              tc_fence_after();
-            }
-            mma_f16_elect(d, da_hi, db_hi, kIdescHead, ks > 0);
-            mma_f16_elect(d, da_lo, db_hi, kIdescHead, 1);
-            mma_f16_elect(d, da_hi, db_lo, kIdescHead, 1);
-            da_hi += 16; da_lo += 16; db_hi += 16; db_lo += 16;
-          }
-          mma_commit_elect(&sc->acc_ready[0]);
-          mma_commit_elect(&sc->acc_ready[1]);
-        }
-        act_phase ^= 1;
-        if (stamp) {
-          P.timeline[6 * tl + 1] = clock64();
-          P.timeline[6 * tl + 4] = si;
-        }
-      }
+  if (warp == kConsumerWarps) {
+    // ===================== producer: L2 -> shared-memory ring (TMA bulk copies) ====================
+    if (lane == 0) {
+      const int64_t total = my_tiles * P.chunks_per_tile;
+      int c = 0;  // chunk index within the per-tile stream
+      for (int64_t g = 0; g < total; ++g) {
+        const int s = (int)(g % kStages);
+        if (g >= kStages) mbar_wait_cluster(&sc->empty[s], (uint32_t)((g / kStages - 1) & 1));
+        mbar_expect_tx(&sc->full[s], kChunkBytes);
+        const unsigned char* src = P.w_tc + (size_t)c * kChunkBytes;
+        const uint32_t dst = smem_u32(ring + s * kChunkBytes);
+        if (PAIR) tma_bulk_g2s_pair(dst + rank * (kChunkBytes / 2), src + rank * (kChunkBytes / 2), kChunkBytes / 2, &sc->full[s]);
+        else tma_bulk_g2s(dst, src, kChunkBytes, &sc->full[s]);
+        if (++c == P.chunks_per_tile) c = 0;
       }
     }
   } else {
-    // ===================== epilogue warps =====================================================
-    const int quarter = warp & 3;        // TMEM lane quarter this warp may access
-    const int half = (warp >> 2) & 1;    // accumulator half (channels 128*half ..) = epilogue group
-    const int shalf = warp >> 3;         // which 16 samples (64 columns) of the tile this warp handles
-    const int ch = 128 * half + 32 * quarter + lane;
-    const uint32_t lane_addr = (uint32_t)(32 * quarter) << 16;
+    // ===================== consumers ===============================================================
+    const int wg = tid >> 7;                                   // channel half
+    const int chb = 128 * wg + 16 * ((tid & 127) >> 5) + (lane >> 2);  // accumulator row (mb, r) = chb + 64 mb + 8 r
+    const int cq = 2 * (lane & 3);                             // first of the two columns in each 8-column block
+    // head mapping: 8 threads per sample s = (row type hj) x (channel half hk)
+    const int hs = tid >> 3, hj = (tid >> 1) & 3, hk = tid & 1;
+    const int hbase = lane & ~7;
     float bad = 0.f;  // max |operand value| seen (fp16 range check)
-    __half2 badh = __floats2half2_rn(0.f, 0.f);  // same for the hidden layers' operands, on packed hi halves
-    uint32_t acc_phase = 0;
+    __half2 badh = __floats2half2_rn(0.f, 0.f);
+    uint32_t peer_empty[kStages];
+#pragma unroll
+    for (int i = 0; i < kStages; ++i) peer_empty[i] = PAIR ? mapa_u32(smem_u32(&sc->empty[i]), rank ^ 1) : 0u;
+    auto release = [&](int64_t g) {
+      if (lane == 0) {
+        const int s = (int)(g % kStages);
+        mbar_arrive(&sc->empty[s]);
+        if (PAIR) mbar_arrive_remote(peer_empty[s]);
+      }
+    };
+    int64_t g = 0;  // chunks consumed
+    HeadOut head;   // distance-side head outputs of sample hs, valid in the threads with hj == 0 && hk == 0
+    std::memset(&head, 0, sizeof(head));
 
-    int gcur = 0;  // geometry buffer of the tile in flight
-    // position embedding of the tile whose geometry is in buffer gcur -> AUX (all four row types)
-    auto prologue_pe = [&]() {
-      asm volatile("bar.sync 1, %0;" ::"n"(kEpiThreads) : "memory");
-      const int s = tid >> 4, sub = tid & 15;
-      write_pos_embedding(p, sc->geo[gcur], aux_hi, aux_lo, s, sub, 16, true, bad);
-      for (int k = p.n_e0 + sub; k < 64; k += 16) store_sample(aux_hi, aux_lo, kAuxK, s, k, 0.f, 0.f, 0.f, 0.f, bad);
-    };
-    auto prologue = [&](int64_t tile) {
-      const int64_t n0 = tile * kTileS;
-      if (tid < kTileS) tile_geometry(p, sc->geo[gcur], n0, tid, n_total);
-      asm volatile("bar.sync 1, %0;" ::"n"(kEpiThreads) : "memory");
-      const int s = tid >> 4, sub = tid & 15;
-      write_pos_embedding(p, sc->geo[gcur], aux_hi, aux_lo, s, sub, 16, true, bad);
-      // zero the K padding of E_s (its weights are zero, the operand must still be finite)
-      for (int k = p.n_e0 + sub; k < 64; k += 16) store_sample(aux_hi, aux_lo, kAuxK, s, k, 0.f, 0.f, 0.f, 0.f, bad);
-    };
-    // colour-trunk inputs E0 | D (| zero pad) into AUX (neddf.py:205-210, 243); 16 threads per sample
-    auto colour_prep = [&]() {
-      const int s = tid >> 4, sub = tid & 15;
-      const int rows = P.eval ? 1 : 4;
-      write_pos_embedding(p, sc->geo[gcur], aux_hi, aux_lo, s, sub, 16, false, bad, rows);
-      const int dhalf = 3 * p.embed_dir;
-      for (int idx = sub; idx < dhalf; idx += 16) {
-        int e = idx / 3, d = idx - 3 * e;
-        float sn, cs;
-        sincosf((float)(1u << e) * sc->geo[gcur][s][3 + d], &sn, &cs);
-        store_sample(aux_hi, aux_lo, kAuxK, s, p.n_e0 + idx, sn, 0.f, 0.f, 0.f, bad, rows);
-        store_sample(aux_hi, aux_lo, kAuxK, s, p.n_e0 + dhalf + idx, cs, 0.f, 0.f, 0.f, bad, rows);
+    for (int64_t t = 0; t < my_tiles; ++t) {
+      const int64_t n0 = tile_of(t) * kTileS;
+      // ---------------- prologue: geometry + scaled position embedding E_s into AUX ---------------
+      if (tid < kTileS) tile_geometry(p, sc->geo, n0, tid, n_total);
+      bar_consumers();
+      {
+        const int s = tid >> 3, sub = tid & 7;
+        write_pos_embedding(p, sc->geo, aux_hi, aux_lo, s, sub, 8, true, bad);
+        // zero the K padding of E_s (its weights are zero, the operand must still be finite)
+        for (int k = p.n_e0 + sub; k < 64; k += 8) store_sample(aux_hi, aux_lo, kAuxK, s, k, 0.f, 0.f, 0.f, 0.f, bad);
       }
-      for (int k = p.n_e0 + p.n_d + 3 + sub; k < kAuxK; k += 16)
-        store_sample(aux_hi, aux_lo, kAuxK, s, k, 0.f, 0.f, 0.f, 0.f, bad, rows);
-    };
-    const bool batched = P.batch > 1;
-    unsigned char* stash = P.stash ? P.stash + (size_t)blockIdx.x * kStashCta : nullptr;
-    auto tile_of = [&](int64_t t) { return (int64_t)blockIdx.x + t * gridDim.x; };
-    // batched mode: the colour inputs E0 | D of the tile's samples go straight to its stash slot (value rows,
-    // operand layout), because AUX already takes the next tile's position embedding while the trunk finishes
-    auto stash_value = [&](unsigned char* slot_aux_hi, int s, int k, float v) {
-      const __half hi = __float2half_rn(v);
-      const __half lo = __float2half_rn(v - __half2float(hi));
-      bad = fmaxf(bad, fabsf(v));
-      const uint32_t off = act_off(s, k, kAuxK);  // rows 0..31: the first four row groups
-      *reinterpret_cast<__half*>(slot_aux_hi + off) = hi;
-      *reinterpret_cast<__half*>(slot_aux_hi + kStashAux + off) = lo;
-    };
-    auto colour_prep_stash = [&](int slot) {
-      unsigned char* a_hi = stash + (size_t)slot * kStashSlot + 2 * kStashH;
-      const int s = tid >> 4, sub = tid & 15;
-      const int half3 = 3 * p.embed_pos;
-      for (int idx = sub; idx < half3; idx += 16) {  // E0: plain position embedding (neddf.py:205-209)
-        int e = idx / 3, d = idx - 3 * e;
-        PeEntry q = pe_entry(e, sc->geo[gcur][s][d], sc->geo[gcur][s][6 + d], p.lowpass[e]);
-        stash_value(a_hi, s, idx, q.scale_0 * q.s);
-        stash_value(a_hi, s, half3 + idx, q.scale_0 * q.c);
-      }
-      const int dhalf = 3 * p.embed_dir;
-      for (int idx = sub; idx < dhalf; idx += 16) {
-        int e = idx / 3, d = idx - 3 * e;
-        float sn, cs;
-        sincosf((float)(1u << e) * sc->geo[gcur][s][3 + d], &sn, &cs);
-        stash_value(a_hi, s, p.n_e0 + idx, sn);
-        stash_value(a_hi, s, p.n_e0 + dhalf + idx, cs);
-      }
-      // (the K padding above n_e0 + n_d + 3 of the stash was zeroed when it was allocated and is never written)
-    };
-    // 16-byte copies between shared memory and the stash, all epilogue threads
-    auto copy_block = [&](unsigned char* dst, const unsigned char* src, uint32_t bytes, bool from_global) {
-      if (from_global) {  // L2 latency: four loads in flight per thread
-        for (uint32_t o = tid * 16; o < bytes; o += 4 * kEpiThreads * 16) {
-          uint4 v[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            if (o + u * kEpiThreads * 16 < bytes) v[u] = __ldcg(reinterpret_cast<const uint4*>(src + o + u * kEpiThreads * 16));
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            if (o + u * kEpiThreads * 16 < bytes) *reinterpret_cast<uint4*>(dst + o + u * kEpiThreads * 16) = v[u];
-        }
-      } else {
-        for (uint32_t o = tid * 16; o < bytes; o += kEpiThreads * 16) *reinterpret_cast<uint4*>(dst + o) = *reinterpret_cast<const uint4*>(src + o);
-      }
-    };
-    if (my_tiles > 0) {
-      prologue(blockIdx.x);
       fence_async_smem();
-      mbar_arrive(&sc->act_ready[half]);
-    }
+      bar_consumers();
 
-    int tl = 0;  // step instance counter (profiling stamps)
-    uint32_t stash_phase = 0;
-    for (int64_t t0 = 0; t0 < my_tiles; t0 += P.batch) {
-      const int ng = (int)((my_tiles - t0 < P.batch) ? my_tiles - t0 : P.batch);
-      for (int ti = 0; ti <= ng; ++ti) {  // ti == ng: the colour steps of the group
-      const int si_begin = ti < ng ? 0 : P.n_trunk, si_end = ti < ng ? P.n_trunk : P.n_steps;
-      // trunk steps: the tile; colour steps of the per-tile program: the same tile (batched: slot k <-> tile t0 + k)
-      const int64_t tile = tile_of(t0 + (ti < ng ? ti : ng - 1));
-      const int64_t n0 = tile * kTileS;
-      const bool more_tiles = t0 + ng < my_tiles;
-      for (int si = si_begin; si < si_end; ++si, ++tl) {
-        const Step& st = P.step[si];
-        const bool more = more_tiles || ti < ng || si + 1 < P.n_steps;  // another step follows
-        // one thread per group polls the mbarrier; the rest sleep in a hardware named barrier
-        if (lane == 0 && quarter == 0 && shalf == 0) mbar_wait(&sc->acc_ready[half], acc_phase);
-        if (half == 0) asm volatile("bar.sync 2, %0;" ::"n"(kEpiThreads / 2) : "memory");
-        else asm volatile("bar.sync 3, %0;" ::"n"(kEpiThreads / 2) : "memory");
-        acc_phase ^= 1;
-        tc_fence_after();
-        const bool stamp = P.timeline && blockIdx.x == 0 && tid == 0 && (tl + 1) * 6 <= P.timeline_cap;
-        if (stamp) P.timeline[6 * tl + 2] = clock64();
-        if (st.kind == kStepHidden) {
-          const float bias = __ldg(P.bias + st.bias_off + ch);
-          const uint32_t tbase = tmem + lane_addr + half * kRows;
-          const bool colour = si > P.head_da_step;
-          const bool value_only = P.eval && colour && !batched;
-          // batched colour layers: the four row blocks are the value rows of four tiles (compiled as a separate
-          // body: sharing one with the trunk's Jacobian rows made every trunk epilogue ~15 % slower)
-          auto hidden_body = [&](auto all_value_tag) {
-          constexpr bool all_value = decltype(all_value_tag)::value;
-#pragma unroll 1
-          for (int blk = (P.debug & 8) ? 2 : 0; blk < 2; ++blk) {  // 8 samples = one 16-byte row group per row type
-            const int s0 = 16 * shalf + 8 * blk;
-            float x[8], d1[8];
-            tmem_ld8(tbase + s0, x);
-            // training: keep the pre-activations [layer][sample][row type][channel] for the backward
-            float* save = nullptr;
-            if (p.save_pre) save = p.save_pre + (((size_t)st.bias_off / kWidth * p.n + (n0 + s0)) * 4) * kWidth + ch;
-            if (save) {
+      for (int l = 0; l < n_hidden; ++l) {
+        const TcLayer L = P.layer[l];
+        const bool vonly = P.eval && l >= p.n_ddf;  // images only: colour trunk on the value rows
+        float acc[2][64];
 #pragma unroll
-              for (int i = 0; i < 8; ++i)
-                if (n0 + s0 + i < n_total) save[(size_t)i * 4 * kWidth] = x[i] + bias;
-            }
+        for (int i = 0; i < 64; ++i) {
+          acc[0][i] = 0.f;
+          acc[1][i] = 0.f;
+        }
+        fence_regs(acc[0]);
+        fence_regs(acc[1]);
+        // ---------------- MMA phase: D_half += W_hi X_hi + W_lo X_hi + W_hi X_lo per K-step -----------
+        const int nk = L.aux_ksteps + L.h_ksteps;
+        for (int ks = 0; ks < nk; ++ks, ++g) {
+          const int s = (int)(g % kStages);
+          mbar_wait(&sc->full[s], (uint32_t)((g / kStages) & 1));
+          const uint32_t w = smem_u32(ring + s * kChunkBytes);
+          uint64_t bhi, blo;
+          if (ks < L.aux_ksteps) {
+            bhi = make_desc(smem_u32(aux_hi) + ks * 256, 128, kAuxK * 16);
+            blo = make_desc(smem_u32(aux_lo) + ks * 256, 128, kAuxK * 16);
+          } else {
+            const int kh = ks - L.aux_ksteps;
+            bhi = make_desc(smem_u32(h_hi) + kh * 256, 128, kHK * 16);
+            blo = make_desc(smem_u32(h_lo) + kh * 256, 128, kHK * 16);
+          }
+          wgmma_fence();
 #pragma unroll
-            for (int i = 0; i < 8; ++i) tc_hidden_act<ACT>(x[i] + bias, x[i], d1[i]);
-            uint32_t h[4], l[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) split2h(x[2 * i], x[2 * i + 1], h[i], l[i], badh);
-            uint32_t off = (uint32_t)((s0 >> 3) * (kHK * 16) + ch * 16);
-            *reinterpret_cast<uint4*>(h_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
-            *reinterpret_cast<uint4*>(h_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
-            if (!value_only) {
-#pragma unroll
-              for (int j = 1; j < 4; ++j) {  // Jacobian rows: G = f'(x) J (tanh_exp.py:47-48)
-                float g[8];
-                tmem_ld8(tbase + 32 * j + s0, g);
-                if (save) {
-#pragma unroll
-                  for (int i = 0; i < 8; ++i)
-                    if (n0 + s0 + i < n_total) save[((size_t)i * 4 + j) * kWidth] = g[i];
-                }
-                if (all_value) {
-                  float dd;
-#pragma unroll
-                  for (int i = 0; i < 8; ++i) tc_hidden_act<ACT>(g[i] + bias, g[i], dd);
-                } else {
-#pragma unroll
-                  for (int i = 0; i < 8; ++i) g[i] *= d1[i];
-                }
-#pragma unroll
-                for (int i = 0; i < 4; ++i) split2h(g[2 * i], g[2 * i + 1], h[i], l[i], badh);
-                off += 4 * (kHK * 16);
-                *reinterpret_cast<uint4*>(h_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
-                *reinterpret_cast<uint4*>(h_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
-              }
+          for (int mb = 0; mb < 2; ++mb) {
+            const uint32_t aoff = (uint32_t)(16 * wg + 8 * mb) * 256;  // 8-channel groups are 256 bytes apart
+            const uint64_t ahi = make_desc(w + aoff, 128, 256), alo = make_desc(w + kChunkBytes / 2 + aoff, 128, 256);
+            if (vonly) {
+              wgmma_n32<0, 1>(acc[mb], ahi, bhi, 1);
+              wgmma_n32<0, 1>(acc[mb], alo, bhi, 1);
+              wgmma_n32<0, 1>(acc[mb], ahi, blo, 1);
+            } else {
+              wgmma_n128<0, 1>(acc[mb], ahi, bhi, 1);
+              wgmma_n128<0, 1>(acc[mb], alo, bhi, 1);
+              wgmma_n128<0, 1>(acc[mb], ahi, blo, 1);
             }
           }
-          };
-          if (batched && colour) hidden_body(std::true_type{});
-          else hidden_body(std::false_type{});
-        } else if (st.kind == kStepHeadDA) {
-          if (warp < 4) {
-            // lane quarter j = row type j, lane = sample: columns 0,1 = ddf_out, aux_out of that row
-            // (neddf.py:220-230); the four types of a sample meet through shared memory
-            float v[4];
-            tmem_ld4(tmem + lane_addr + kHeadCol, v);
-            sc->hgather[quarter][lane][0] = v[0];
-            sc->hgather[quarter][lane][1] = v[1];
-            asm volatile("bar.sync 4, 128;" ::: "memory");
-            if (warp == 0) {
-              const int s = lane;
-              float ddf[4], aux[4];
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                ddf[j] = sc->hgather[j][s][0];
-                aux[j] = sc->hgather[j][s][1];
-              }
-              ddf[0] += __ldg(p.b_head + 0);
-              aux[0] += __ldg(p.b_head + 1);
-              HeadOut h;
-              head_density(ddf, aux, p.d_near, p.aux_grad_scale, p.density_act, h);
-              const int kn = p.n_e0 + p.n_d;  // normal: detached, zero Jacobian (neddf.py:243-253)
-              if (batched) {
-                // images only: the distance-side outputs leave now, the normal joins the parked colour inputs
-                unsigned char* a_hi = stash + (size_t)ti * kStashSlot + 2 * kStashH;
-#pragma unroll
-                for (int i = 0; i < 3; ++i) stash_value(a_hi, s, kn + i, h.normal[i]);
-                const int64_t n = n0 + s;
-                if (n < n_total) {
-                  int64_t ray_, on;
-                  int j_;
-                  field_map(p, n, ray_, j_, on);
-                  if (p.distance) p.distance[on] = h.distance;
-                  if (p.density) p.density[on] = h.density;
-                  if (p.aux_grad) p.aux_grad[on] = h.aux;
-                }
-              } else {
-                sc->head[s] = h;
-#pragma unroll
-                for (int i = 0; i < 3; ++i)
-                  store_sample(aux_hi, aux_lo, kAuxK, s, kn + i, h.normal[i], 0.f, 0.f, 0.f, bad, P.eval ? 1 : 4);
-              }
-            }
+          wgmma_commit();
+          if (ks > 0) {
+            wgmma_wait<1>();
+            release(g - 1);
           }
-          if (batched) {
-            // park the value rows of the tile's features (rows 0..31 = the first four row groups of H)
-            asm volatile("bar.sync 1, %0;" ::"n"(kEpiThreads) : "memory");  // the last trunk layer's rows, all threads'
-            unsigned char* slot = stash + (size_t)ti * kStashSlot;
-            copy_block(slot, h_hi, kStashH, false);
-            copy_block(slot + kStashH, h_lo, kStashH, false);
-            if (ti + 1 == ng) {
-              __threadfence();  // this thread's parked rows (plain global stores) before the others read them back
-              // group complete: every slot comes back as rows 32 slot + sample of H and AUX (the heads' MMAs have
-              // finished reading H: their commit is what released this epilogue)
-              asm volatile("bar.sync 1, %0;" ::"n"(kEpiThreads) : "memory");
-              // (all slots, also those a short last group does not use: their rows are old but finite, whereas
-              // never-written shared memory could trip the fp16 range check).  One thread issues the bulk copies.
-              if (tid == 0) {
-                fence_async_all();  // the parked rows were written with ordinary stores
-                mbar_expect_tx(&sc->stash_bar, (uint32_t)P.batch * kStashSlot);
-                for (int k = 0; k < P.batch; ++k) {
-                  const unsigned char* src = stash + (size_t)k * kStashSlot;
-                  tma_bulk_g2s(smem_u32(h_hi + k * kStashH), src, kStashH, &sc->stash_bar);
-                  tma_bulk_g2s(smem_u32(h_lo + k * kStashH), src + kStashH, kStashH, &sc->stash_bar);
-                  tma_bulk_g2s(smem_u32(aux_hi + k * kStashAux), src + 2 * kStashH, kStashAux, &sc->stash_bar);
-                  tma_bulk_g2s(smem_u32(aux_lo + k * kStashAux), src + 2 * kStashH + kStashAux, kStashAux, &sc->stash_bar);
+        }
+        wgmma_wait<0>();
+        fence_regs(acc[0]);
+        fence_regs(acc[1]);
+        release(g - 1);
+        bar_consumers();  // both warpgroups are done reading H / AUX
+
+        // ---------------- epilogue: bias + activation + Jacobian, next layer's operand into H ---------
+        const float* bias = P.bias + (size_t)l * kWidth;
+#pragma unroll
+        for (int mb = 0; mb < 2; ++mb) {
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const int ch = chb + 64 * mb + 8 * r;
+            const float b = __ldg(bias + ch);
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {  // samples 8q + cq, 8q + cq + 1
+              float y[2], d1[2];
+              const uint32_t off = (uint32_t)(q * (kHK * 16) + ch * 16 + cq * 2);
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const float xpre = acc[mb][4 * q + 2 * r + e] + b;
+                if (p.save_pre) {  // training: keep the pre-activations [layer][sample][row type][channel]
+                  const int64_t n = n0 + 8 * q + cq + e;
+                  if (n < n_total) {
+                    float* dst = p.save_pre + (((size_t)l * p.n + n) * 4) * kWidth + ch;
+                    dst[0] = xpre;
+#pragma unroll
+                    for (int j = 1; j < 4; ++j) dst[j * kWidth] = acc[mb][16 * j + 4 * q + 2 * r + e];
+                  }
+                }
+                tc_hidden_act<ACT>(xpre, y[e], d1[e]);
+              }
+              uint32_t hi, lo;
+              split2h(y[0], y[1], hi, lo, badh);
+              *reinterpret_cast<uint32_t*>(h_hi + off) = hi;
+              *reinterpret_cast<uint32_t*>(h_lo + off) = lo;
+              if (!vonly) {
+#pragma unroll
+                for (int j = 1; j < 4; ++j) {  // Jacobian rows: G = f'(x) J (tanh_exp.py:47-48)
+                  const float g0 = d1[0] * acc[mb][16 * j + 4 * q + 2 * r];
+                  const float g1 = d1[1] * acc[mb][16 * j + 4 * q + 2 * r + 1];
+                  split2h(g0, g1, hi, lo, badh);
+                  *reinterpret_cast<uint32_t*>(h_hi + off + j * 4 * (kHK * 16)) = hi;
+                  *reinterpret_cast<uint32_t*>(h_lo + off + j * 4 * (kHK * 16)) = lo;
                 }
               }
-              if (lane == 0) mbar_wait(&sc->stash_bar, stash_phase);
-              __syncwarp();
-              stash_phase ^= 1;
-            }
-          } else if (st.post == 1) {
-            colour_prep();  // only when no earlier MMA phase could hide it
-          }
-        } else if (batched) {
-          // colour head of the group (neddf.py:257): lane quarter = slot, lane = sample
-          if (warp < 4 && quarter < ng) {
-            float v[4];
-            tmem_ld4(tmem + lane_addr + kHeadCol, v);
-            const int64_t n = tile_of(t0 + quarter) * kTileS + lane;
-            if (n < n_total && p.color) {
-              int64_t ray_, on;
-              int j_;
-              field_map(p, n, ray_, j_, on);
-              p.color[3 * on + 0] = v[0] + __ldg(p.b_head + 2);
-              p.color[3 * on + 1] = v[1] + __ldg(p.b_head + 3);
-              p.color[3 * on + 2] = v[2] + __ldg(p.b_head + 4);
-            }
-          }
-        } else {
-          // colour head (neddf.py:257) + penalties (:259-300) + outputs
-          if (warp < 4) {
-            float v[4];
-            tmem_ld4(tmem + lane_addr + kHeadCol, v);
-            sc->hgather[quarter][lane][0] = v[0];
-            sc->hgather[quarter][lane][1] = v[1];
-            sc->hgather[quarter][lane][2] = v[2];
-            asm volatile("bar.sync 4, 128;" ::: "memory");
-            const int s = lane;
-            const int64_t n = n0 + s;
-            if (warp == 0 && n < n_total) {
-              const HeadOut& h = sc->head[s];
-              float col[3], colJ[3][3];
-#pragma unroll
-              for (int c = 0; c < 3; ++c) {
-                col[c] = sc->hgather[0][s][c] + __ldg(p.b_head + 2 + c);
-#pragma unroll
-                for (int i = 0; i < 3; ++i) colJ[i][c] = sc->hgather[1 + i][s][c];
-              }
-              int64_t ray_, on;  // where this sample's outputs go (segment view: [ray, edge] of the full arrays)
-              int j_;
-              field_map(p, n, ray_, j_, on);
-              if (p.distance) p.distance[on] = h.distance;
-              if (p.density) p.density[on] = h.density;
-              if (p.aux_grad) p.aux_grad[on] = h.aux;
-              if (p.color) {
-                p.color[3 * on + 0] = col[0];
-                p.color[3 * on + 1] = col[1];
-                p.color[3 * on + 2] = col[2];
-              }
-              // (in images-only mode the colour Jacobian rows are not computed and no penalty is asked)
-              if (p.penalty) p.penalty[on] = field_penalty(h, col, colJ, p.distance_range_max, p.penalty_weight);
             }
           }
         }
-        tc_fence_before();
-        fence_async_smem();
-        if (stamp) {
-          P.timeline[6 * tl + 3] = clock64();
-          P.timeline[6 * tl + 5] = si;
-        }
-        if (more) mbar_arrive(&sc->act_ready[half]);
-        // work that only feeds later steps runs here, under the next step's MMA phase; its
-        // shared-memory writes are published by the fence + arrive of the following steps
-        if (batched && ti < ng) {
-          // spread over the trunk so that each piece hides under one layer's MMAs: this tile's colour inputs early,
-          // the next tile's position embedding once AUX is free
-          // (a scattered global write of 2-byte values and a prologue are ~4k cycles each: together they did not fit
-          // under one layer, and the embedding written to global memory instead of AUX took 11k)
-          if (si == 1) {
-            colour_prep_stash(ti);
-            // the next tile's geometry (dependent global loads) into the other buffer, long before it is needed
-            if (ti + 1 < ng && tid < kTileS) tile_geometry(p, sc->geo[gcur ^ 1], tile_of(t0 + ti + 1) * kTileS, tid, n_total);
+        bar_consumers();
+
+        // row hj of sample hs in H, channel half hk; the start is rotated so that the 8 threads of a sample
+        // read different bank groups
+        const int hrow = 32 * hj + hs;
+        const uint32_t hrow_off = (uint32_t)((hrow >> 3) * (kHK * 16) + (hrow & 7) * 2);
+        const int rot = hj + 4 * hk;
+        auto hval = [&](int k) {
+          return __half2float(*reinterpret_cast<const __half*>(h_hi + hrow_off + k * 16)) +
+                 __half2float(*reinterpret_cast<const __half*>(h_lo + hrow_off + k * 16));
+        };
+        if (l == p.n_ddf - 1) {
+          // ------------ distance / aux heads (neddf.py:220-241) + colour-trunk inputs ---------------
+          float pd = 0.f, pa = 0.f;
+#pragma unroll 4
+          for (int kk = 0; kk < 128; ++kk) {
+            const int k = 128 * hk + ((kk + rot) & 127);
+            const float v = hval(k);
+            const float2 wv = __ldg(reinterpret_cast<const float2*>(p.w_head_da) + k);
+            pd = fmaf(v, wv.x, pd);
+            pa = fmaf(v, wv.y, pa);
           }
-          if (st.kind == kStepHidden && st.post == 1 && ti + 1 < ng) {  // AUX is free from here
-            gcur ^= 1;
-            prologue_pe();
+          pd += __shfl_xor_sync(0xffffffffu, pd, 1);
+          pa += __shfl_xor_sync(0xffffffffu, pa, 1);
+          float ddf[4], aux[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            ddf[j] = __shfl_sync(0xffffffffu, pd, hbase + 2 * j);
+            aux[j] = __shfl_sync(0xffffffffu, pa, hbase + 2 * j);
           }
-        } else if (st.kind == kStepHidden && st.post == 1) {
-          colour_prep();
-        }
-        if (st.post == 2) {
-          if (batched) {
-            if (more_tiles) prologue(tile_of(t0 + ng));
-          } else if (more_tiles) {
-            prologue(tile_of(t0 + 1));
+          const int rows = P.eval ? 1 : 4;
+          if (hj == 0 && hk == 0) {
+            ddf[0] += __ldg(p.b_head + 0);
+            aux[0] += __ldg(p.b_head + 1);
+            head_density(ddf, aux, p.d_near, p.aux_grad_scale, p.density_act, head);
+            const int kn = p.n_e0 + p.n_d;  // normal: detached, zero Jacobian (neddf.py:243-253)
+#pragma unroll
+            for (int i = 0; i < 3; ++i) store_sample(aux_hi, aux_lo, kAuxK, hs, kn + i, head.normal[i], 0.f, 0.f, 0.f, bad, rows);
+          }
+          // colour-trunk inputs E0 | D (| zero pad) into AUX (neddf.py:205-210, 243); the trunk is done with E_s
+          {
+            const int s = tid >> 3, sub = tid & 7;
+            write_pos_embedding(p, sc->geo, aux_hi, aux_lo, s, sub, 8, false, bad, rows);
+            const int dhalf = 3 * p.embed_dir;
+            for (int idx = sub; idx < dhalf; idx += 8) {
+              int e = idx / 3, d = idx - 3 * e;
+              float sn, cs;
+              sincosf((float)(1u << e) * sc->geo[s][3 + d], &sn, &cs);
+              store_sample(aux_hi, aux_lo, kAuxK, s, p.n_e0 + idx, sn, 0.f, 0.f, 0.f, bad, rows);
+              store_sample(aux_hi, aux_lo, kAuxK, s, p.n_e0 + dhalf + idx, cs, 0.f, 0.f, 0.f, bad, rows);
+            }
+            for (int k = p.n_e0 + p.n_d + 3 + sub; k < kAuxK; k += 8)
+              store_sample(aux_hi, aux_lo, kAuxK, s, k, 0.f, 0.f, 0.f, 0.f, bad, rows);
+          }
+          bar_consumers();
+        } else if (l == n_hidden - 1) {
+          // ------------ colour head (neddf.py:257) + penalties (:259-300) + outputs ----------------
+          float pc[3] = {0.f, 0.f, 0.f};
+          if (!P.eval || hj == 0) {
+#pragma unroll 4
+            for (int kk = 0; kk < 128; ++kk) {
+              const int k = 128 * hk + ((kk + rot) & 127);
+              const float v = hval(k);
+              const float4 wv = __ldg(reinterpret_cast<const float4*>(p.w_head_col) + k);
+              pc[0] = fmaf(v, wv.x, pc[0]);
+              pc[1] = fmaf(v, wv.y, pc[1]);
+              pc[2] = fmaf(v, wv.z, pc[2]);
+            }
+          }
+          float colv[4][3];
+#pragma unroll
+          for (int c = 0; c < 3; ++c) {
+            pc[c] += __shfl_xor_sync(0xffffffffu, pc[c], 1);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) colv[j][c] = __shfl_sync(0xffffffffu, pc[c], hbase + 2 * j);
+          }
+          const int64_t n = n0 + hs;
+          if (hj == 0 && hk == 0 && n < n_total) {
+            float col[3], colJ[3][3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+              col[c] = colv[0][c] + __ldg(p.b_head + 2 + c);
+#pragma unroll
+              for (int i = 0; i < 3; ++i) colJ[i][c] = colv[1 + i][c];
+            }
+            int64_t ray_, on;  // where this sample's outputs go (segment view: [ray, edge] of the full arrays)
+            int j_;
+            field_map(p, n, ray_, j_, on);
+            if (p.distance) p.distance[on] = head.distance;
+            if (p.density) p.density[on] = head.density;
+            if (p.aux_grad) p.aux_grad[on] = head.aux;
+            if (p.color) {
+              p.color[3 * on + 0] = col[0];
+              p.color[3 * on + 1] = col[1];
+              p.color[3 * on + 2] = col[2];
+            }
+            // (in images-only mode the colour Jacobian rows are not computed and no penalty is asked)
+            if (p.penalty) p.penalty[on] = field_penalty(head, col, colJ, p.distance_range_max, p.penalty_weight);
           }
         }
-      }
+        fence_async_smem();  // this layer's operand writes -> the next MMAs (async proxy)
+        bar_consumers();
       }
     }
-    {
-      const float2 m = __half22float2(badh);
-      if (!(fmaxf(bad, fmaxf(m.x, m.y)) < 65504.0f) && P.status) atomicOr(P.status, 4);
-    }
+    const float2 m = __half22float2(badh);
+    if (!(fmaxf(bad, fmaxf(m.x, m.y)) < 65504.0f) && P.status) atomicOr(P.status, 4);
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp) tmem_dealloc(tmem, kTmemCols);
+  // a CTA of a pair leaves only when its partner can no longer arrive on its barriers
+  if (PAIR) cluster_sync_all();
 }
 
 // ---------------------------------------------------------------------------------------------
 // weight packing: fp32 [in,out] -> fp16 hi/lo chunks in consumption order
 // ---------------------------------------------------------------------------------------------
 struct TcPackArgs {
-  const float* w[kMaxHidden + 3];
-  const float* b[kMaxHidden + 3];
+  const float* w[kMaxHidden];
+  const float* b[kMaxHidden];
   int k_in[kMaxHidden];
   int aux_real[kMaxHidden];  // leading input channels that live in AUX (0 if none)
   int aux_pad[kMaxHidden];   // their padded K extent in AUX
   int ksteps[kMaxHidden];
-  int chunk0[kMaxHidden + 3];  // first chunk index of the layer / head
+  int chunk0[kMaxHidden];    // first chunk index of the layer
   int n_hidden;
 };
 
-// Consumption order of a hidden layer's chunks.  K-steps split into G0 = [AUX steps + first half
-// of the H steps] and G1 = [second half of the H steps]; the MMA warp issues
-// (half 0, G0), (half 1, G0), (half 0, G1), (half 1, G1) so that channel half 0 completes a quarter
-// layer before half 1 and the two epilogue groups can trail the tensor core (see the kernel).
-__host__ __device__ __forceinline__ int chunk_pos(int ksteps, int aux_ksteps, int ks, int half) {
-  const int n1 = (ksteps - aux_ksteps) / 2, n0 = ksteps - n1;
-  return (ks < n0) ? half * n0 + ks : 2 * n0 + half * n1 + (ks - n0);
-}
-
 __global__ void tc_pack_hidden_kernel(TcPackArgs a, unsigned char* __restrict__ dst, float* __restrict__ bias) {
   const int l = blockIdx.y;
-  const int total = a.ksteps[l] * 2 * 128 * 16;  // (kstep, half, m, k)
+  const int total = a.ksteps[l] * kWidth * 16;  // (kstep, m, k)
   for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
-    int k = idx & 15, m = (idx >> 4) & 127, half = (idx >> 11) & 1, ks = idx >> 12;
-    int kk = ks * 16 + k;  // K index in operand space (AUX part first, then H)
-    int row;               // reference weight row, -1 = zero padding
+    const int k = idx & 15, m = (idx >> 4) & (kWidth - 1), ks = idx >> 12;
+    const int kk = ks * 16 + k;  // K index in operand space (AUX part first, then H)
+    int row;                     // reference weight row, -1 = zero padding
     if (kk < a.aux_pad[l]) row = (kk < a.aux_real[l]) ? kk : -1;
     else row = a.aux_real[l] + (kk - a.aux_pad[l]);
     if (row >= a.k_in[l]) row = -1;
-    float w = (row >= 0) ? a.w[l][(size_t)row * kWidth + 128 * half + m] : 0.f;
-    __half hi = __float2half_rn(w);
-    __half lo = __float2half_rn(w - __half2float(hi));
-    unsigned char* chunk = dst + (size_t)(a.chunk0[l] + chunk_pos(a.ksteps[l], a.aux_pad[l] / 16, ks, half)) * kChunkBytes;
-    // tensor-memory A layout: row m = lane, k pairs packed per 32-bit column; 8 hi words then 8 lo words
-    *reinterpret_cast<__half*>(chunk + m * 64 + k * 2) = hi;
-    *reinterpret_cast<__half*>(chunk + m * 64 + 32 + k * 2) = lo;
+    const float w = (row >= 0) ? a.w[l][(size_t)row * kWidth + m] : 0.f;
+    const __half hi = __float2half_rn(w);
+    const __half lo = __float2half_rn(w - __half2float(hi));
+    unsigned char* chunk = dst + (size_t)(a.chunk0[l] + ks) * kChunkBytes;
+    *reinterpret_cast<__half*>(chunk + wchunk_off(m, k)) = hi;
+    *reinterpret_cast<__half*>(chunk + kChunkBytes / 2 + wchunk_off(m, k)) = lo;
   }
   if (blockIdx.x == 0)
     for (int c = threadIdx.x; c < kWidth; c += blockDim.x) bias[l * kWidth + c] = a.b[l][c];
-}
-
-// heads: chunk0[n_hidden] = (ddf,aux) hi chunk, +1 lo; chunk0[n_hidden+1] = colour hi, +1 lo
-__global__ void tc_pack_heads_kernel(TcPackArgs a, unsigned char* __restrict__ dst) {
-  const int nh = a.n_hidden;
-  for (int idx = threadIdx.x; idx < 16 * kWidth; idx += blockDim.x) {
-    int k = idx % kWidth, n = idx / kWidth;
-    float wda = (n == 0) ? a.w[nh + 0][k] : (n == 1) ? a.w[nh + 1][k] : 0.f;
-    float wc = (n < 3) ? a.w[nh + 2][3 * k + n] : 0.f;
-    __half h1 = __float2half_rn(wda), h2 = __float2half_rn(wc);
-    __half l1 = __float2half_rn(wda - __half2float(h1)), l2 = __float2half_rn(wc - __half2float(h2));
-    *reinterpret_cast<__half*>(dst + (size_t)a.chunk0[nh] * kStageBytes + hchunk_off(n, k)) = h1;
-    *reinterpret_cast<__half*>(dst + (size_t)(a.chunk0[nh] + 1) * kStageBytes + hchunk_off(n, k)) = l1;
-    *reinterpret_cast<__half*>(dst + (size_t)a.chunk0[nh + 1] * kStageBytes + hchunk_off(n, k)) = h2;
-    *reinterpret_cast<__half*>(dst + (size_t)(a.chunk0[nh + 1] + 1) * kStageBytes + hchunk_off(n, k)) = l2;
-  }
 }
 
 struct TcStorage {
   unsigned char* d_w = nullptr;
   float* d_bias = nullptr;
   int* d_status = nullptr;
-  int n_steps = 0;
   int chunks_per_tile = 0;
-  Step step[kMaxSteps];
+  TcLayer layer[kMaxHidden];
   TcPackArgs pack;
-  long long* timeline = nullptr;
-  int timeline_cap = 0;
-  int head_da_step = 0;
-  int chunks_trunk = 0;
-  unsigned char* d_stash = nullptr;  // batched colour trunk: parked value rows, kMaxBatch slots per CTA
 };
 
 // ---------------------------------------------------------------------------------------------
-// self-test of the MMA building block (pins descriptor / layout conventions on hardware)
+// self-test of the MMA building block (pins descriptor / layout conventions on hardware):
+// C[m, n] = sum_k A[m, k] B[n, k], A K-major weight chunks, B MN-major activations, m = 128
 // ---------------------------------------------------------------------------------------------
-// n == 128: hidden configuration.  C[m, n] = sum_k A[m,k] B[n,k], A = "weights" (K-major chunks),
-//           B = "activations" (MN-major in H).
-// n == 16 : head configuration.    C[m, n] = sum_k A[m,k] B[n,k], A = "activations" (MN-major in H),
-//           B = "head weights" (K-major chunk).
-__global__ void __launch_bounds__(128, 1) tc_selftest_kernel(const float* __restrict__ A, const float* __restrict__ B,
-                                                             int n, int k, float* __restrict__ C) {
+template <int N>
+__global__ void __launch_bounds__(256, 1) tc_selftest_kernel(const float* __restrict__ A, const float* __restrict__ B, int k,
+                                                            float* __restrict__ C) {
   extern __shared__ __align__(1024) unsigned char smem[];
-  unsigned char* h_hi = smem;                 // 64 KB
-  unsigned char* h_lo = smem + kHBytes;       // 64 KB
-  unsigned char* w_hi = smem + 2 * kHBytes;   // up to 8 chunks of 4 KB (hidden, k <= 128) or 8 KB (head)
-  unsigned char* w_lo = w_hi + 32768;
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_base;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const bool hidden = (n == kRows);
-  // operands -> fp16 hi/lo in the kernel layouts
-  for (int idx = tid; idx < 128 * k; idx += 128) {
-    int kk = idx % k, r = idx / k;
-    float a = A[(size_t)r * k + kk];
-    __half hi = __float2half_rn(a), lo = __float2half_rn(a - __half2float(hi));
-    if (hidden) {  // A = weights: chunk per k-step of 16, 4 KB each
-      uint32_t off = (uint32_t)(kk >> 4) * 4096 + wchunk_off(r, kk & 15);
-      *reinterpret_cast<__half*>(w_hi + off) = hi;
-      *reinterpret_cast<__half*>(w_lo + off) = lo;
-    } else {       // A = activations in H
-      *reinterpret_cast<__half*>(h_hi + act_off(r, kk, kHK)) = hi;
-      *reinterpret_cast<__half*>(h_lo + act_off(r, kk, kHK)) = lo;
-    }
+  // A: per K-step the m < 128 half of a weight chunk (hi 4 KB | lo 4 KB); B: [n/8][k][n%8], K capacity k
+  constexpr int kA = kChunkBytes / 2;
+  const int ksteps = k / 16;
+  unsigned char* a_buf = smem;
+  unsigned char* b_hi = smem + (size_t)ksteps * kA;
+  unsigned char* b_lo = b_hi + (size_t)N * k * 2;
+  const int tid = threadIdx.x;
+  for (int i = tid; i < 128 * k; i += blockDim.x) {
+    const int m = i / k, kk = i % k;
+    const float v = A[i];
+    const __half hi = __float2half_rn(v), lo = __float2half_rn(v - __half2float(hi));
+    unsigned char* chunk = a_buf + (size_t)(kk / 16) * kA;
+    *reinterpret_cast<__half*>(chunk + wchunk_off(m, kk & 15)) = hi;
+    *reinterpret_cast<__half*>(chunk + kA / 2 + wchunk_off(m, kk & 15)) = lo;
   }
-  for (int idx = tid; idx < n * k; idx += 128) {
-    int kk = idx % k, r = idx / k;
-    float b = B[(size_t)r * k + kk];
-    __half hi = __float2half_rn(b), lo = __float2half_rn(b - __half2float(hi));
-    if (hidden) {
-      *reinterpret_cast<__half*>(h_hi + act_off(r, kk, kHK)) = hi;
-      *reinterpret_cast<__half*>(h_lo + act_off(r, kk, kHK)) = lo;
-    } else {
-      *reinterpret_cast<__half*>(w_hi + hchunk_off(r, kk)) = hi;
-      *reinterpret_cast<__half*>(w_lo + hchunk_off(r, kk)) = lo;
-    }
+  for (int i = tid; i < N * k; i += blockDim.x) {
+    const int n = i / k, kk = i % k;
+    const float v = B[i];
+    const __half hi = __float2half_rn(v), lo = __float2half_rn(v - __half2float(hi));
+    *reinterpret_cast<__half*>(b_hi + act_off(n, kk, k)) = hi;
+    *reinterpret_cast<__half*>(b_lo + act_off(n, kk, k)) = lo;
   }
-  if (tid == 0) {
-    mbar_init(&bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) tmem_alloc(&tmem_base, 128);
   fence_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_base;
-  if (tid == 0) {
-    const uint32_t s_hhi = smem_u32(h_hi), s_hlo = smem_u32(h_lo), s_whi = smem_u32(w_hi), s_wlo = smem_u32(w_lo);
-    for (int ks = 0; ks < k / 16; ++ks) {
-      if (hidden) {
-        uint64_t da_hi = make_desc(s_whi + ks * 4096, 128, 256), da_lo = make_desc(s_wlo + ks * 4096, 128, 256);
-        uint64_t db_hi = make_desc(s_hhi + ks * 256, 128, kHK * 16), db_lo = make_desc(s_hlo + ks * 256, 128, kHK * 16);
-        mma_f16(tmem, da_hi, db_hi, kIdescHidden, ks > 0);
-        mma_f16(tmem, da_lo, db_hi, kIdescHidden, 1);
-        mma_f16(tmem, da_hi, db_lo, kIdescHidden, 1);
+  if (tid < 128 * 2) {
+    const int wg = tid >> 7, lane = tid & 31;
+    constexpr int R = N / 2;
+    float acc[R];
+#pragma unroll
+    for (int i = 0; i < R; ++i) acc[i] = 0.f;
+    fence_regs(acc);
+    wgmma_fence();
+    for (int ks = 0; ks < ksteps; ++ks) {
+      const uint32_t w = smem_u32(a_buf + (size_t)ks * kA) + (uint32_t)(8 * wg) * 256;
+      const uint64_t ahi = make_desc(w, 128, 256), alo = make_desc(w + kA / 2, 128, 256);
+      const uint64_t bhi = make_desc(smem_u32(b_hi) + ks * 256, 128, k * 16), blo = make_desc(smem_u32(b_lo) + ks * 256, 128, k * 16);
+      if constexpr (N == 128) {
+        wgmma_n128<0, 1>(acc, ahi, bhi, 1);
+        wgmma_n128<0, 1>(acc, alo, bhi, 1);
+        wgmma_n128<0, 1>(acc, ahi, blo, 1);
       } else {
-        uint64_t da_hi = make_desc(s_hhi + ks * 256, 128, kHK * 16), da_lo = make_desc(s_hlo + ks * 256, 128, kHK * 16);
-        uint64_t db_hi = make_desc(s_whi + ks * 256, 128, 4096), db_lo = make_desc(s_wlo + ks * 256, 128, 4096);
-        mma_f16(tmem, da_hi, db_hi, kIdescHead, ks > 0);
-        mma_f16(tmem, da_lo, db_hi, kIdescHead, 1);
-        mma_f16(tmem, da_hi, db_lo, kIdescHead, 1);
+        wgmma_n16<0, 1>(acc, ahi, bhi, 1);
+        wgmma_n16<0, 1>(acc, alo, bhi, 1);
+        wgmma_n16<0, 1>(acc, ahi, blo, 1);
       }
     }
-    mma_commit(&bar);
-  }
-  mbar_wait(&bar, 0);
-  tc_fence_after();
-  // lane = row m of D; columns = n
-  const int m = 32 * warp + lane;
-  for (int cb = 0; cb < n / 16; ++cb) {
-    float v[16];
-    tmem_ld16(tmem + ((uint32_t)(32 * warp) << 16) + cb * 16, v);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(acc);
+    const int row = 64 * wg + 16 * ((tid & 127) >> 5) + (lane >> 2);
 #pragma unroll
-    for (int i = 0; i < 16; ++i) C[(size_t)m * n + cb * 16 + i] = v[i];
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, 128);
-}
-
-// TS-mode self-test: C[m, n] = sum_k A[m,k] B[n,k] with A (weights) written to tensor memory by
-// tcgen05.st and B (activations, MN-major) in shared memory; m = n = 128.
-__global__ void __launch_bounds__(128, 1) tc_selftest_ts_kernel(const float* __restrict__ A,
-                                                                const float* __restrict__ B, int k,
-                                                                float* __restrict__ C, long long* __restrict__ cyc,
-                                                                int reps) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  unsigned char* h_hi = smem;
-  unsigned char* h_lo = smem + kHBytes;
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_base;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  for (int idx = tid; idx < 128 * k; idx += 128) {
-    int kk = idx % k, r = idx / k;
-    float b = B[(size_t)r * k + kk];
-    __half hi = __float2half_rn(b), lo = __float2half_rn(b - __half2float(hi));
-    *reinterpret_cast<__half*>(h_hi + act_off(r, kk, kHK)) = hi;
-    *reinterpret_cast<__half*>(h_lo + act_off(r, kk, kHK)) = lo;
-  }
-  if (tid == 0) {
-    mbar_init(&bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) tmem_alloc(&tmem_base, 512);
-  fence_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_base;
-  // A: lane = row m; per K-step 8 columns hi at 256 + ks*16, 8 columns lo right after
-  const int m = 32 * warp + lane;
-  for (int ks = 0; ks < k / 16; ++ks) {
-    uint32_t hi[8], lo[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float a0 = A[(size_t)m * k + ks * 16 + 2 * j], a1 = A[(size_t)m * k + ks * 16 + 2 * j + 1];
-      float amax = 0.f;
-      split2(a0, a1, hi[j], lo[j], amax);
-    }
-    const uint32_t ta = tmem + ((uint32_t)(32 * warp) << 16) + 256 + ks * 16;
-    tmem_st8(ta, hi);
-    tmem_st8(ta + 8, lo);
-  }
-  tmem_st_wait();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 0) {
-    const uint32_t s_hhi = smem_u32(h_hi), s_hlo = smem_u32(h_lo);
-    long long t0 = clock64();
-    for (int r = 0; r < reps; ++r) {
-      for (int ks = 0; ks < k / 16; ++ks) {
-        const uint64_t db_hi = make_desc(s_hhi + ks * 256, 128, kHK * 16), db_lo = make_desc(s_hlo + ks * 256, 128, kHK * 16);
-        const uint32_t ta = tmem + 256 + ks * 16;
-        mma_f16_ts_elect(tmem, ta, db_hi, kIdescHidden, (r | ks) > 0);
-        mma_f16_ts_elect(tmem, ta + 8, db_hi, kIdescHidden, 1);
-        mma_f16_ts_elect(tmem, ta, db_lo, kIdescHidden, 1);
-      }
-    }
-    mma_commit_elect(&bar);
-    mbar_wait(&bar, 0);
-    long long t1 = clock64();
-    if (lane == 0 && cyc) cyc[0] = t1 - t0;
-  }
-  __syncthreads();
-  tc_fence_after();
-  for (int cb = 0; cb < 128 / 16; ++cb) {
-    float v[16];
-    tmem_ld16(tmem + ((uint32_t)(32 * warp) << 16) + cb * 16, v);
-#pragma unroll
-    for (int i = 0; i < 16; ++i) C[(size_t)m * 128 + cb * 16 + i] = v[i] / (float)reps;
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, 512);
-}
-
-// ---------------------------------------------------------------------------------------------
-// MMA issue-rate microbenchmark: `reps` x 16 back-to-back MMAs on garbage operands in shared
-// memory, timed with clock64() between the first issue and the commit's arrival.
-//   a_mn, b_mn  : operand majorness (0 = K-major, 1 = MN-major)
-//   swz         : 0 = no swizzle (LBO 128), 2 = SWIZZLE_128B
-//   n           : MMA N (M is 128)
-// ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 1) tc_mma_bench_kernel(int a_mn, int b_mn, int swz, int n, int reps,
-                                                              long long* __restrict__ out) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  __shared__ uint64_t bar, bar2;
-  __shared__ uint32_t tmem_base;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  if (tid == 0) mbar_init(&bar2, 1 << 20);
-  for (int i = tid; i < 49152; i += 128) reinterpret_cast<uint32_t*>(smem)[i] = 0x3c003c00u;  // 1.0h
-  if (tid == 0) {
-    mbar_init(&bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) tmem_alloc(&tmem_base, 512);
-  fence_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_base;
-  if (tid == 0) {
-    const uint32_t sa = smem_u32(smem), sb = smem_u32(smem) + 65536;
-    const uint32_t idesc = make_idesc(128, n, a_mn, b_mn);
-    const uint64_t lay = (uint64_t)(swz & 7) << 61;
-    long long t0 = clock64();
-    for (int r = 0; r < reps; ++r) {
-#pragma unroll 1
-      for (int ks = 0; ks < 16; ++ks) {
-        // operand strides as the megakernel uses them (no swizzle) or the canonical SW128 ones
-        uint64_t da, db;
-        if (swz == 0) {
-          da = a_mn ? make_desc(sa + ks * 256, 128, 4096) : make_desc(sa + ks * 4096, 128, 256);
-          db = b_mn ? make_desc(sb + ks * 256, 128, 4096 * (n > 128 ? 1 : 1)) : make_desc(sb + ks * 4096, 128, 256);
-        } else {
-          da = make_desc(sa + ks * 32, 16, 1024) | lay;
-          db = make_desc(sb + ks * 32, 16, 1024) | lay;
-        }
-        if (swz < 8) {
-          mma_f16(tmem + (ks & 1) * 256, da, db, idesc, 1);
-        } else {
-          // megakernel issue pattern: wide (N=256) + narrow (N=128) MMA per chunk, commit per chunk
-          const int pat = swz - 8;
-          mma_f16(tmem + (ks & 1) * 256, make_desc(sa + ks * 4096, 128, 256), make_desc(sb + ks * 256, 128, 4096),
-                  make_idesc(128, 256, 0, 1), 1);
-          mma_f16(tmem + (ks & 1) * 256, make_desc(sa + ks * 4096 + 2048, 128, 256), make_desc(sb + ks * 256, 128, 4096),
-                  (pat & 1) ? make_idesc(128, 256, 0, 1) : make_idesc(128, 128, 0, 1), 1);
-          if (pat & 2) mma_commit(&bar2);
-        }
-      }
-    }
-    mma_commit(&bar);
-    long long t1 = clock64();
-    mbar_wait(&bar, 0);
-    long long t2 = clock64();
-    if (blockIdx.x == 0) {
-      out[0] = t1 - t0;
-      out[1] = t2 - t0;
+    for (int i = 0; i < R; ++i) {
+      const int m = row + 8 * ((i >> 1) & 1), n = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+      C[(size_t)m * N + n] = acc[i];
     }
   }
-  __syncthreads();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, 512);
 }
 
 }  // namespace tc
@@ -1102,18 +599,18 @@ static bool is_skip_layer(const neddf_field* f, int l) {
   return false;
 }
 
+// both engines ("tc" and its CTA-pair form "tc2") cover any embedding ranks whose inputs fit AUX (64 K of E_s,
+// 96 K of E0 | D | n) and 256-wide layers
 bool tc_supported(const neddf_field* f) {
-  // built for the reference network shape: 60-channel position embedding, 24-channel direction
-  // embedding (AUX holds 64 / 96 K), 256-wide layers
-  return f->cfg.embed_pos_rank == 10 && f->cfg.embed_dir_rank == 4 && f->cfg.ddf_layer_width == kWidth &&
-         f->cfg.col_layer_width == kWidth;
+  const int n_e0 = 6 * f->cfg.embed_pos_rank, off_h = n_e0 + 6 * f->cfg.embed_dir_rank + 3;
+  return n_e0 <= 64 && off_h <= tc::kAuxK && f->cfg.ddf_layer_width == kWidth && f->cfg.col_layer_width == kWidth;
 }
 
 static int32_t tc_ensure(neddf_field* f) {
   if (f->tc) return NEDDF_OK;
   tc::TcStorage* S = new tc::TcStorage();
   const int n_hidden = f->n_ddf + f->n_col;
-  int chunk = 0, si = 0;
+  int chunk = 0;
   std::memset(&S->pack, 0, sizeof(S->pack));
   S->pack.n_hidden = n_hidden;
   for (int l = 0; l < n_hidden; ++l) {
@@ -1122,58 +619,24 @@ static int32_t tc_ensure(neddf_field* f) {
     else if (l < f->n_ddf) { if (is_skip_layer(f, l)) { aux_real = f->proto.n_e0; aux_pad = 64; } h_k = kWidth; }
     else if (l == f->n_ddf) { aux_real = f->proto.off_h; aux_pad = tc::kAuxK; h_k = kWidth; }
     else h_k = kWidth;
-    tc::Step& st = S->step[si++];
-    st.kind = tc::kStepHidden;
-    st.aux_ksteps = aux_pad / 16;
-    st.h_ksteps = h_k / 16;
-    st.bias_off = l * kWidth;
-    st.post = 0;
+    S->layer[l].aux_ksteps = aux_pad / 16;
+    S->layer[l].h_ksteps = h_k / 16;
     S->pack.k_in[l] = f->shape_in[l];
     S->pack.aux_real[l] = aux_real;
     S->pack.aux_pad[l] = aux_pad;
-    S->pack.ksteps[l] = st.aux_ksteps + st.h_ksteps;
+    S->pack.ksteps[l] = S->layer[l].aux_ksteps + S->layer[l].h_ksteps;
     S->pack.chunk0[l] = chunk;
-    chunk += 2 * S->pack.ksteps[l];
-    if (l == f->n_ddf - 1) {  // distance / aux heads after the trunk
-      tc::Step& hs = S->step[si++];
-      hs.kind = tc::kStepHeadDA; hs.aux_ksteps = 0; hs.h_ksteps = kWidth / 16; hs.bias_off = 0; hs.post = 0;
-    }
+    chunk += S->pack.ksteps[l];
   }
-  tc::Step& cs = S->step[si++];
-  cs.kind = tc::kStepHeadCol; cs.aux_ksteps = 0; cs.h_ksteps = kWidth / 16; cs.bias_off = 0; cs.post = 0;
-  // the four head-weight chunks ((ddf,aux) hi, lo, colour hi, lo) follow the streamed chunks; the
-  // kernel copies them to shared memory once
-  S->pack.chunk0[n_hidden] = chunk;
-  S->pack.chunk0[n_hidden + 1] = chunk + 2;
-  S->n_steps = si;
   S->chunks_per_tile = chunk;
-  {
-    // AUX holds E_s until the last trunk layer that reads it (layer 0 or the last skip consumer);
-    // after that layer's epilogue the colour inputs E0|D can be written while later trunk layers
-    // run.  If that layer is the last trunk layer the heads step does it inline.
-    int last_aux = 0, head_da = -1, first_col = -1;
-    for (int i = 0; i < si; ++i) {
-      if (S->step[i].kind == tc::kStepHeadDA) head_da = i;
-      if (head_da < 0 && S->step[i].kind == tc::kStepHidden && S->step[i].aux_ksteps > 0) last_aux = i;
-      if (head_da >= 0 && first_col < 0 && S->step[i].kind == tc::kStepHidden) first_col = i;
-    }
-    S->head_da_step = head_da;
-    S->chunks_trunk = S->pack.chunk0[f->n_ddf];
-    if (last_aux + 1 < head_da) S->step[last_aux].post = 1;
-    else S->step[head_da].post = 1;
-    // after the first colour layer's epilogue AUX is dead again: next tile's prologue goes there
-    S->step[first_col].post = 2;
-  }
-  if (cudaMalloc(&S->d_w, (size_t)(chunk + 4) * tc::kChunkBytes) != cudaSuccess ||
+  if (cudaMalloc(&S->d_w, (size_t)chunk * tc::kChunkBytes) != cudaSuccess ||
       cudaMalloc(&S->d_bias, (size_t)n_hidden * kWidth * sizeof(float)) != cudaSuccess ||
-      cudaMalloc(&S->d_status, sizeof(int)) != cudaSuccess ||
-      cudaMalloc(&S->d_stash, (size_t)sm_count() * tc::kStashCta) != cudaSuccess) {
-    cudaFree(S->d_w); cudaFree(S->d_bias); cudaFree(S->d_status); cudaFree(S->d_stash);
+      cudaMalloc(&S->d_status, sizeof(int)) != cudaSuccess) {
+    cudaFree(S->d_w); cudaFree(S->d_bias); cudaFree(S->d_status);
     delete S;
     return fail(NEDDF_E_CUDA, "tensor-core engine: cudaMalloc failed");
   }
   cudaMemset(S->d_status, 0, sizeof(int));
-  cudaMemset(S->d_stash, 0, (size_t)sm_count() * tc::kStashCta);  // the K padding of the parked colour inputs stays zero
   f->tc = S;
   return NEDDF_OK;
 }
@@ -1184,7 +647,6 @@ void tc_destroy(neddf_field* f) {
   cudaFree(S->d_w);
   cudaFree(S->d_bias);
   cudaFree(S->d_status);
-  cudaFree(S->d_stash);
   delete S;
   f->tc = nullptr;
 }
@@ -1195,74 +657,57 @@ int32_t tc_pack_weights(neddf_field* f, const float* const* d_w, const float* co
   tc::TcStorage* S = static_cast<tc::TcStorage*>(f->tc);
   tc::TcPackArgs a = S->pack;
   const int n_hidden = f->n_ddf + f->n_col;
-  for (int l = 0; l < n_hidden + 3; ++l) {
+  for (int l = 0; l < n_hidden; ++l) {
     a.w[l] = d_w[l];
     a.b[l] = d_b[l];
   }
   tc::tc_pack_hidden_kernel<<<dim3(64, n_hidden), 256, 0, s>>>(a, S->d_w, S->d_bias);
   NEDDF_LAUNCH_CHECK();
-  tc::tc_pack_heads_kernel<<<1, 256, 0, s>>>(a, S->d_w);
-  NEDDF_LAUNCH_CHECK();
   return NEDDF_OK;
 }
 
-int32_t launch_field_tc(const neddf_field* f, FieldParams& p, int flags, cudaStream_t s) {
+int32_t launch_field_tc(const neddf_field* f, FieldParams& p, int flags, bool pair, cudaStream_t s) {
   tc::TcStorage* S = static_cast<tc::TcStorage*>(f->tc);
   if (!S) return fail(NEDDF_E_INVALID, "tensor-core engine: weights were never packed");
   tc::TcParams P;
   P.f = p;
-  P.n_steps = S->n_steps;
+  for (int l = 0; l < p.n_ddf + p.n_col; ++l) P.layer[l] = S->layer[l];
   P.chunks_per_tile = S->chunks_per_tile;
-  for (int i = 0; i < S->n_steps; ++i) P.step[i] = S->step[i];
   P.w_tc = S->d_w;
   P.bias = S->d_bias;
   P.status = S->d_status;
-  P.eval = (flags == NEDDF_OUT_EVAL && p.penalty == nullptr) ? 1 : 0;
-  P.head_da_step = S->head_da_step;
-  P.n_trunk = S->head_da_step + 1;
-  P.chunks_trunk = S->chunks_trunk;
-  // images only: one colour-trunk pass per four tiles (NEDDF_TC_BATCH=1 keeps the per-tile program)
-  // (needs the trunk's last reader of AUX to be hidden layer 2 or later: the hooks that hide the per-tile work sit
-  // under layer 1 and that one)
-  bool can_batch = false;
-  for (int i = 2; i < S->head_da_step; ++i) can_batch = can_batch || (S->step[i].kind == tc::kStepHidden && S->step[i].post == 1);
-  P.batch = (P.eval && p.save_pre == nullptr && can_batch) ? tc::kMaxBatch : 1;
-  if (const char* e = std::getenv("NEDDF_TC_BATCH")) P.batch = std::max(1, std::min(P.batch, std::atoi(e)));
-  P.stash = S->d_stash;
-  P.debug = 0;
-  if (const char* e = std::getenv("NEDDF_TC_DEBUG")) {
-    P.debug = std::atoi(e);
-    static bool warned = false;
-    if (P.debug && !warned) {
-      warned = true;
-      std::fprintf(stderr, "neddf_b200: NEDDF_TC_DEBUG=%d switches kernel stages off - timing only, results are garbage\n", P.debug);
-    }
-  }
-  P.timeline = S->timeline;
-  P.timeline_cap = S->timeline_cap;
-  int64_t n_tiles = (p.n + tc::kTileS - 1) / tc::kTileS;
-  int grid = (int)std::min<int64_t>(n_tiles, sm_count());
+  P.eval = (flags == NEDDF_OUT_EVAL && p.penalty == nullptr && p.save_pre == nullptr) ? 1 : 0;
+  const int64_t n_tiles = (p.n + tc::kTileS - 1) / tc::kTileS;
   auto launch = [&](auto kern) -> int32_t {
     NEDDF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::kSmemBytes));
-    kern<<<grid, tc::kThreads, tc::kSmemBytes, s>>>(P);
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr[1];
+    cfg.blockDim = dim3(tc::kThreads);
+    cfg.dynamicSmemBytes = tc::kSmemBytes;
+    cfg.stream = s;
+    if (pair) {
+      const int64_t pairs = (n_tiles + 1) / 2;
+      cfg.gridDim = dim3((unsigned)(2 * std::max<int64_t>(1, std::min<int64_t>(pairs, sm_count() / 2))));
+      attr[0].id = cudaLaunchAttributeClusterDimension;
+      attr[0].val.clusterDim.x = 2;
+      attr[0].val.clusterDim.y = 1;
+      attr[0].val.clusterDim.z = 1;
+      cfg.attrs = attr;
+      cfg.numAttrs = 1;
+    } else {
+      cfg.gridDim = dim3((unsigned)std::max<int64_t>(1, std::min<int64_t>(n_tiles, sm_count())));
+      cfg.numAttrs = 0;
+    }
+    NEDDF_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, P));
     NEDDF_LAUNCH_CHECK();
     return NEDDF_OK;
   };
   switch (p.hidden_act) {
-    case NEDDF_ACT_TANHEXP: return launch(tc::field_tc_kernel<NEDDF_ACT_TANHEXP>);
-    case NEDDF_ACT_RELU: return launch(tc::field_tc_kernel<NEDDF_ACT_RELU>);
-    case NEDDF_ACT_LEAKYRELU: return launch(tc::field_tc_kernel<NEDDF_ACT_LEAKYRELU>);
+    case NEDDF_ACT_TANHEXP: return pair ? launch(tc::field_tc_kernel<NEDDF_ACT_TANHEXP, true>) : launch(tc::field_tc_kernel<NEDDF_ACT_TANHEXP, false>);
+    case NEDDF_ACT_RELU: return pair ? launch(tc::field_tc_kernel<NEDDF_ACT_RELU, true>) : launch(tc::field_tc_kernel<NEDDF_ACT_RELU, false>);
+    case NEDDF_ACT_LEAKYRELU: return pair ? launch(tc::field_tc_kernel<NEDDF_ACT_LEAKYRELU, true>) : launch(tc::field_tc_kernel<NEDDF_ACT_LEAKYRELU, false>);
   }
   return fail(NEDDF_E_INVALID, "tensor-core engine: unknown activation");
-}
-
-int32_t tc_set_timeline(neddf_field* f, long long* d_buf, int cap) {
-  int32_t rc = tc_ensure(f);
-  if (rc != NEDDF_OK) return rc;
-  tc::TcStorage* S = static_cast<tc::TcStorage*>(f->tc);
-  S->timeline = d_buf;
-  S->timeline_cap = d_buf ? cap : 0;
-  return NEDDF_OK;
 }
 
 int32_t tc_read_status(const neddf_field* f, int* out, cudaStream_t s) {
@@ -1277,41 +722,18 @@ int32_t tc_read_status(const neddf_field* f, int* out, cudaStream_t s) {
 
 }  // namespace neddf
 
-extern "C" int32_t neddf_tc_mma_bench(int32_t a_mn, int32_t b_mn, int32_t swizzle, int32_t n, int32_t reps,
-                                      int64_t* d_cycles, void* stream) {
-  using namespace neddf;
-  if (!d_cycles || reps < 1 || n < 16 || n > 256 || (n % 16)) return fail(NEDDF_E_INVALID, "neddf_tc_mma_bench: bad arguments");
-  size_t smem = 196608;
-  NEDDF_CUDA_CHECK(cudaFuncSetAttribute(tc::tc_mma_bench_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int grid = 1;
-  if (const char* e = std::getenv("NEDDF_MMA_BENCH_GRID")) grid = std::max(1, std::atoi(e));
-  tc::tc_mma_bench_kernel<<<grid, 128, smem, (cudaStream_t)stream>>>(a_mn, b_mn, swizzle, n, reps,
-                                                                 reinterpret_cast<long long*>(d_cycles));
-  NEDDF_LAUNCH_CHECK();
-  return NEDDF_OK;
-}
-
-extern "C" int32_t neddf_tc_selftest_ts(const float* d_a, const float* d_b, int32_t k, float* d_c, int64_t* d_cycles,
-                                        int32_t reps, void* stream) {
-  using namespace neddf;
-  if (k < 16 || k > 256 || (k % 16) != 0 || reps < 1) return fail(NEDDF_E_INVALID, "neddf_tc_selftest_ts: bad k / reps");
-  if (!d_a || !d_b || !d_c) return fail(NEDDF_E_INVALID, "neddf_tc_selftest_ts: NULL pointer");
-  size_t smem = 2 * tc::kHBytes;
-  NEDDF_CUDA_CHECK(cudaFuncSetAttribute(tc::tc_selftest_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  tc::tc_selftest_ts_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(d_a, d_b, k, d_c, reinterpret_cast<long long*>(d_cycles), reps);
-  NEDDF_LAUNCH_CHECK();
-  return NEDDF_OK;
-}
-
 extern "C" int32_t neddf_tc_selftest(const float* d_a, const float* d_b, int32_t m, int32_t n, int32_t k, float* d_c,
                                      void* stream) {
   using namespace neddf;
-  if (m != 128 || (n != 128 && n != 16) || k < 16 || k > (n == 128 ? 128 : 256) || (k % 16) != 0)
+  if (m != 128 || (n != 128 && n != 16) || k < 16 || (k % 16) != 0 || k > (n == 128 ? 128 : 256))
     return fail(NEDDF_E_INVALID, "neddf_tc_selftest: need m=128, n in {128,16}, k multiple of 16 (<=128 for n=128, <=256 for n=16)");
   if (!d_a || !d_b || !d_c) return fail(NEDDF_E_INVALID, "neddf_tc_selftest: NULL pointer");
-  size_t smem = 2 * tc::kHBytes + 65536;
-  NEDDF_CUDA_CHECK(cudaFuncSetAttribute(tc::tc_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  tc::tc_selftest_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(d_a, d_b, n, k, d_c);
-  NEDDF_LAUNCH_CHECK();
-  return NEDDF_OK;
+  const size_t smem = (size_t)(k / 16) * (tc::kChunkBytes / 2) + (size_t)2 * n * k * 2;
+  auto launch = [&](auto kern) -> int32_t {
+    NEDDF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<1, 256, smem, (cudaStream_t)stream>>>(d_a, d_b, k, d_c);
+    NEDDF_LAUNCH_CHECK();
+    return NEDDF_OK;
+  };
+  return n == 128 ? launch(tc::tc_selftest_kernel<128>) : launch(tc::tc_selftest_kernel<16>);
 }

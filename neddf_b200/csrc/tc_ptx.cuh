@@ -1,5 +1,5 @@
-// tcgen05 / TMEM / mbarrier PTX wrappers, operand layouts and the split-fp16 helpers shared by the
-// tensor-core field kernels (field_tc.cu: one CTA per SM; field_tc2.cu: CTA pairs, cta_group::2).
+// Hopper (sm_90a) building blocks of the tensor-core kernels (field_tc.cu, wgrad.cu): wgmma / mbarrier /
+// TMA bulk-copy wrappers, operand layouts and the split-fp16 helpers.
 #pragma once
 
 #include "field_math.cuh"
@@ -10,27 +10,23 @@ namespace neddf {
 namespace tc {
 
 constexpr int kTileS = 32;              // samples per CTA tile
-constexpr int kRows = 4 * kTileS;       // 128 = MMA N (hidden) / M (heads)
+constexpr int kRows = 4 * kTileS;       // 128 = MMA N (hidden layers)
 constexpr int kHK = 256;                // K capacity of H
 constexpr int kAuxK = 96;               // K capacity of AUX
-constexpr int kChunkBytes = 8192;       // one weight chunk: 128 rows x (8 words hi | 8 words lo)
+constexpr int kChunkBytes = 16384;      // one weight chunk: 16 K x 256 channels, fp16 hi (8 KB) | lo (8 KB)
 constexpr uint32_t kHBytes = kRows * kHK * 2;      // 65536 per hi / lo
 constexpr uint32_t kAuxBytes = kRows * kAuxK * 2;  // 24576 per hi / lo
 
 // ---------------------------------------------------------------------------------------------
-// layouts
+// layouts (canonical no-swizzle wgmma layouts: 8 x 16-byte core matrices)
 // ---------------------------------------------------------------------------------------------
-// B/A operand, MN-major, no swizzle: element (row, k) of a buffer with K capacity KC
+// activations, MN-major: element (row, k) of a buffer with K capacity KC at [row/8][k][row%8]
 __host__ __device__ __forceinline__ uint32_t act_off(int row, int k, int KC) {
   return (uint32_t)((row >> 3) * (KC * 16) + k * 16 + (row & 7) * 2);
 }
-// weight chunk (K-major, no swizzle): [m/8][k/8][m%8][k%8] fp16, m in [0,128), k in [0,16)
+// weight chunk, K-major: [m/8][k/8][m%8][k%8] fp16, m in [0,256), k in [0,16)
 __host__ __device__ __forceinline__ uint32_t wchunk_off(int m, int k) {
   return (uint32_t)((m >> 3) * 256 + (k >> 3) * 128 + (m & 7) * 16 + (k & 7) * 2);
-}
-// head-weight chunk (K-major): [n/8][k/8][n%8][k%8] fp16, n in [0,16), k in [0,256)
-__host__ __device__ __forceinline__ uint32_t hchunk_off(int n, int k) {
-  return (uint32_t)((n >> 3) * 4096 + (k >> 3) * 128 + (n & 7) * 16 + (k & 7) * 2);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -58,157 +54,85 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
 }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(cols)
+// TMA 1-D bulk copy global -> shared memory, completion counted in bytes on an mbarrier
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void tma_bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem),
+               "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
 }
 
-// shared-memory matrix descriptor, SWIZZLE_NONE, version 1 (cute::UMMA::SmemDescriptor)
+// wgmma shared-memory matrix descriptor, no swizzle: start, leading (K-direction) and stride (M/N-direction)
+// byte offsets between core matrices
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFFu);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
-// instruction descriptor, kind::f16: fp16 x fp16 -> fp32 (cute::UMMA::InstrDescriptor)
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
-}
-constexpr uint32_t kIdescHidden = make_idesc(128, kRows, 0, 1);      // A weights K-major, B activations MN-major
-constexpr uint32_t kIdescHiddenValue = make_idesc(128, kTileS, 0, 1);  // value rows only (eval colour trunk)
-constexpr uint32_t kIdescHead = make_idesc(kRows, 16, 1, 0);     // A activations MN-major, B head weights K-major
 
-__device__ __forceinline__ void mma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// A operand from tensor memory ("TS"): A[m][k] lives in lane m, 32-bit column k/2 (two fp16 per
-// column, even k in the low half) - cute::UMMA::tmem_frg_1sm<half_t>.
-__device__ __forceinline__ void mma_f16_ts_elect(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, q;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, {%5, %5, %5, %5}, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(0u)
-      : "memory");
-}
-// One weight chunk: D += A_hi*B_hi + A_lo*B_hi + A_hi*B_lo (A_hi at TMEM columns a..a+7, A_lo at a+8..),
-// then tcgen05.commit to `bar` (shared-memory address) - one elected lane, one asm block.
-__device__ __forceinline__ void chunk_mma_elect(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_hi, uint64_t b_lo,
-                                                uint32_t idesc, uint32_t accumulate, uint32_t bar) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, q, t;\n"
-      ".reg .b32 alo;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "setp.ne.b32 p, %5, 0;\n"
-      "setp.ne.b32 t, %8, 0;\n"
-      "add.u32 alo, %1, 8;\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %4, {%7, %7, %7, %7}, p;\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [alo], %2, %4, {%7, %7, %7, %7}, t;\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %3, %4, {%7, %7, %7, %7}, t;\n"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%6];\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_hi), "l"(b_lo), "r"(idesc), "r"(accumulate), "r"(bar), "r"(0u), "r"(1u)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t r[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t a[8], const uint32_t b[8]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(a[4]), "r"(a[5]), "r"(a[6]), "r"(a[7]), "r"(b[0]), "r"(b[1]), "r"(b[2]),
-      "r"(b[3]), "r"(b[4]), "r"(b[5]), "r"(b[6]), "r"(b[7])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// Warp-uniform variants: the whole warp executes them with identical operands and one elected
-// lane issues.  Keeping the issuing code convergent lets ptxas hold descriptors in uniform
-// registers; under `if (lane == 0)` it wraps every UTCHMMA in an ELECT/R2UR.BROADCAST loop.
-__device__ __forceinline__ void mma_f16_elect(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, q;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_commit_elect(uint64_t* bar) {
-  asm volatile(
-      "{\n"
-      ".reg .pred q;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n"
-      "}\n" ::"r"(smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float v[16]) {
-  uint32_t r[16];
+// m64nNk16, fp16 x fp16 -> fp32, A and B from shared memory.  TA / TB: 0 = K-major, 1 = MN-major.
+// Accumulator fragment (thread t of the warpgroup, register i):
+//   row = 16 (t / 32) + (t % 32) / 4 + 8 ((i / 2) % 2),  column = 8 (i / 4) + 2 (t % 4) + i % 2
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-      "tcgen05.wait::ld.sync.aligned;\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float v[8]) {
-  uint32_t r[8];
+// (the first 16 registers of an n128 accumulator: columns 0..31)
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n32(float* d, uint64_t a, uint64_t b, uint32_t acc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];\n"
-      "tcgen05.wait::ld.sync.aligned;\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %19, %20;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, float v[4]) {
-  uint32_t r[4];
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];\n"
-      "tcgen05.wait::ld.sync.aligned;\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 4; ++i) v[i] = __uint_as_float(r[i]);
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,"
+      "%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,"
+      "%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
+        "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
+        "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+        "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1, %131, %132;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
 }
 
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -292,165 +216,6 @@ __device__ __forceinline__ void store_sample(unsigned char* hi_buf, unsigned cha
     *reinterpret_cast<uint16_t*>(hi_buf + off + 3 * tstride) = (uint16_t)(h1 >> 16);
     *reinterpret_cast<uint16_t*>(lo_buf + off + 3 * tstride) = (uint16_t)(l1 >> 16);
   }
-}
-
-// Sum v[i] over the 32 lanes of the warp for N values per lane; afterwards lane L holds the totals of
-// indices [L * N / 32, (L + 1) * N / 32) in v[0 .. N/32).  N / 32 * 31 shuffles instead of 5 N.
-template <int N>
-__device__ __forceinline__ void warp_transpose_reduce(float (&v)[N], int lane) {
-#pragma unroll
-  for (int d = 16, n = N / 2; d >= 1; d >>= 1, n >>= 1) {
-    const bool upper = (lane & d) != 0;
-#pragma unroll
-    for (int t = 0; t < n; ++t) {
-      const float send = upper ? v[t] : v[t + n];
-      const float keep = upper ? v[t + n] : v[t];
-      v[t] = keep + __shfl_xor_sync(0xffffffffu, send, d);
-    }
-  }
-}
-
-// N = 16: lane L ends with the total of index L >> 1 (both lanes of a pair hold it)
-__device__ __forceinline__ void warp_transpose_reduce16(float (&v)[16], int lane) {
-#pragma unroll
-  for (int d = 16, n = 8; d >= 2; d >>= 1, n >>= 1) {
-    const bool upper = (lane & d) != 0;
-#pragma unroll
-    for (int t = 0; t < n; ++t) {
-      const float send = upper ? v[t] : v[t + n];
-      const float keep = upper ? v[t + n] : v[t];
-      v[t] = keep + __shfl_xor_sync(0xffffffffu, send, d);
-    }
-  }
-  v[0] += __shfl_xor_sync(0xffffffffu, v[0], 1);
-}
-
-// ---------------------------------------------------------------------------------------------
-// CTA pairs: clusters of two CTAs on one TPC, tcgen05 cta_group::2
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t cluster_id_x() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `saddr` (a shared::cta address of this CTA) in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t saddr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void st_cluster_v2(uint32_t caddr, uint2 v) {
-  asm volatile("st.shared::cluster.v2.b32 [%0], {%1,%2};" ::"r"(caddr), "r"(v.x), "r"(v.y) : "memory");
-}
-__device__ __forceinline__ void st_cluster_v4(uint32_t caddr, uint4 v) {
-  asm volatile("st.shared::cluster.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(caddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ void st_cluster_f32(uint32_t caddr, float v) {
-  asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(caddr), "f"(v) : "memory");
-}
-// arrive (release at cluster scope) on an mbarrier given by its shared::cluster address
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t caddr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(caddr) : "memory");
-}
-// arrive without any memory fence (the data handed over is tensor memory, ordered by tcgen05 fences, or
-// was already published by an explicit fence)
-__device__ __forceinline__ void mbar_arrive_cluster_relaxed(uint32_t caddr) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(caddr) : "memory");
-}
-// default semantics (release at CTA scope): what CUTLASS's ClusterBarrier::arrive(cta_id) uses for DSMEM hand-offs
-__device__ __forceinline__ void mbar_arrive_cluster_default(uint32_t caddr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(caddr) : "memory");
-}
-// four 8-column loads in flight, one wait (lane = TMEM lane, 4 x 8 consecutive columns at taddr + stride * j)
-__device__ __forceinline__ void tmem_ld8x4(uint32_t t0, uint32_t t1, uint32_t t2, uint32_t t3, float a[8], float b[8], float c[8], float d[8]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%32];\n"
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%8,%9,%10,%11,%12,%13,%14,%15}, [%33];\n"
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%16,%17,%18,%19,%20,%21,%22,%23}, [%34];\n"
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%24,%25,%26,%27,%28,%29,%30,%31}, [%35];\n"
-      "tcgen05.wait::ld.sync.aligned;\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(t0), "r"(t1), "r"(t2), "r"(t3)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    a[i] = __uint_as_float(r[i]);
-    b[i] = __uint_as_float(r[8 + i]);
-    c[i] = __uint_as_float(r[16 + i]);
-    d[i] = __uint_as_float(r[24 + i]);
-  }
-}
-__device__ __forceinline__ void fence_acq_rel_cluster() { asm volatile("fence.acq_rel.cluster;" ::: "memory"); }
-// wait with acquire at cluster scope (the barrier is local; the arrivals may come from the peer CTA)
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "TC_WAITC:\n"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra TC_DONEC;\n"
-      "bra TC_WAITC;\n"
-      "TC_DONEC:\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
-// TMA 1-D bulk copy global -> shared memory, completion counted in bytes on an mbarrier
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tma_bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem),
-               "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void fence_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_alloc2(uint32_t* dst_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t addr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
-}
-// M = 256 (128 rows of A / D per CTA), A from each CTA's tensor memory, B split between the CTAs
-__device__ __forceinline__ void mma2_f16_ts_elect(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                                  uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, q;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "@q tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(0u)
-      : "memory");
-}
-// commit of all prior cta_group::2 MMAs to the mbarrier at the same shared-memory offset in the CTAs of `mask`
-__device__ __forceinline__ void mma2_commit_elect(uint32_t bar, uint32_t mask) {
-  asm volatile(
-      "{\n"
-      ".reg .pred q;\n"
-      ".reg .b16 lo, hi;\n"
-      "mov.b32 {lo, hi}, %1;\n"
-      "elect.sync _|q, 0xffffffff;\n"
-      "@q tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], lo;\n"
-      "}\n" ::"r"(bar),
-      "r"(mask)
-      : "memory");
 }
 
 }  // namespace tc

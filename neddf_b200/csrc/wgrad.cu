@@ -9,13 +9,13 @@
 // (cuBLAS); this kernel keeps the training path free of library GEMMs.
 //
 // Per CTA: one 128-column tile of A (M = 128), all 256 columns of B (N = 256), a contiguous slab of rows.
-// Eight producer warps stream 64-row stages from HBM (row pieces of 128 B per quarter-warp), split every
+// Two warpgroups (256 threads) stream 64-row stages from HBM (row pieces of 128 B per quarter-warp), split every
 // fp32 value into fp16 hi + lo on the fly and store both operands MN-major in shared memory
-// ([column / 8][row][column % 8], conflict-free 16-byte stores).  One thread issues, per 16 rows,
-//     D += A_hi^T B_hi + A_lo^T B_hi + A_hi^T B_lo        (tcgen05.mma kind::f16, M 128 x N 256 x K 16,
-// both operands from shared memory: at N = 256 the SS form runs at the tensor floor, tools/mma_bench.py),
-// fp32 accumulation in tensor memory (256 columns).  The slab's partial result goes to a workspace and a
-// second kernel adds the slabs in a fixed order (deterministic gradients, no atomics).
+// ([column / 8][row][column % 8], conflict-free 16-byte stores), double-buffered so that the conversion of
+// stage s + 1 overlaps the MMAs of stage s.  Warpgroup g accumulates columns [64g, 64g + 64) of A, per 16 rows
+//     D += A_hi^T B_hi + A_lo^T B_hi + A_hi^T B_lo        (wgmma m64n256k16 f16, both operands MN-major)
+// in 128 fp32 registers per thread.  The slab's partial result goes to a workspace and a second kernel adds
+// the slabs in a fixed order (deterministic gradients, no atomics).
 //
 // The bias gradient (sum of gy over the value rows) is a column sum: colsum_rows_kernel + the same reducer.
 #include "tc_ptx.cuh"
@@ -34,16 +34,9 @@ constexpr int kTileN = 256;                       // columns of B
 constexpr uint32_t kABytes = kTileM * kStageRows * 2;  // 16 KB per hi / lo
 constexpr uint32_t kBBytes = kTileN * kStageRows * 2;  // 32 KB per hi / lo
 constexpr uint32_t kStageBytes = 2 * kABytes + 2 * kBBytes;  // 96 KB
-constexpr int kProdWarps = 8;
-constexpr int kThreads = (kProdWarps + 1) * 32;   // + one MMA / epilogue-control warp (warp 8)
-constexpr uint32_t kSmemBytes = kStages * kStageBytes + 256;
-
-struct Bars {
-  uint64_t full[kStages];   // producers -> MMA: stage converted and stored
-  uint64_t empty[kStages];  // tcgen05.commit -> producers: stage consumed
-  uint64_t done;            // tcgen05.commit -> everyone: accumulator complete
-  uint32_t tmem_base;
-};
+constexpr int kWarps = 8;
+constexpr int kThreads = kWarps * 32;
+constexpr uint32_t kSmemBytes = kStages * kStageBytes;
 
 // 8 consecutive fp32 -> 8 fp16 hi (16 bytes) + 8 fp16 lo
 __device__ __forceinline__ void split8(const float4& a, const float4& b, uint4& hi, uint4& lo) {
@@ -68,122 +61,91 @@ __global__ void __launch_bounds__(kThreads, 1)
     wgrad_gemm_kernel(const float* __restrict__ A, int64_t lda, int a_col0, int ka, const float* __restrict__ B, int64_t ldb,
                       int64_t rows, int64_t rows_per_slab, float* __restrict__ partial) {
   extern __shared__ __align__(1024) unsigned char smem[];
-  Bars* bars = reinterpret_cast<Bars*>(smem + kStages * kStageBytes);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
   const int64_t r_begin = (int64_t)blockIdx.x * rows_per_slab;
   const int64_t r_end = min(rows, r_begin + rows_per_slab);
   const int64_t n_stage = (r_end > r_begin) ? (r_end - r_begin + kStageRows - 1) / kStageRows : 0;
 
-  if (tid == 0) {
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(&bars->full[s], kProdWarps * 32);  // every producer thread after its own writes
-      mbar_init(&bars->empty[s], 1);
-    }
-    mbar_init(&bars->done, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == kProdWarps) tmem_alloc(&bars->tmem_base, 256);
-  fence_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars->tmem_base;
-
-  if (warp < kProdWarps) {
-    // ---------------- producers: HBM -> fp16 hi / lo, MN-major operands --------------------------
-    // a warp instruction covers 8 rows x 4 column groups of 8: lane = 8 * group + row, so a quarter-warp
-    // stores 8 consecutive rows of one column group (128 contiguous bytes of shared memory) and the four
-    // quarter-warps read one 128-byte piece of each of the 8 rows
-    const int lr = lane & 7, lg = lane >> 3;
-    for (int64_t it = 0; it < n_stage; ++it) {
-      const int s = (int)(it % kStages);
-      if (it >= kStages) mbar_wait(&bars->empty[s], (uint32_t)((it / kStages - 1) & 1));
-      unsigned char* st = smem + s * kStageBytes;
-      unsigned char* a_hi = st;
-      unsigned char* a_lo = st + kABytes;
-      unsigned char* b_hi = st + 2 * kABytes;
-      unsigned char* b_lo = st + 2 * kABytes + kBBytes;
-      const int64_t r0 = r_begin + it * kStageRows;
-      // units: A has 8 row blocks x 4 group blocks (of 4 groups), B has 8 x 8; 96 units over 8 warps
-      for (int u = warp; u < 96; u += kProdWarps) {
-        const bool isA = u < 32;
-        const int uu = isA ? u : u - 32;
-        const int rb = uu & 7, gb = uu >> 3;
-        const int row = 8 * rb + lr;            // row within the stage = K index
-        const int grp = 4 * gb + lg;            // column group of 8 = MN index / 8
-        const int64_t r = r0 + row;
-        float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
-        if (r < r_end) {
-          if (isA) {
-            const int c = 8 * grp;
-            if (c + 8 <= ka && ((lda | a_col0) & 3) == 0) {
-              const float4* src = reinterpret_cast<const float4*>(A + r * lda + a_col0 + c);
-              v0 = __ldg(src);
-              v1 = __ldg(src + 1);
-            } else if (c < ka) {  // ragged edge / unaligned rows (k_in = 60, 87; the 2- and 4-column heads)
-              float t[8];
+  float acc[128];
 #pragma unroll
-              for (int i = 0; i < 8; ++i) t[i] = (c + i < ka) ? __ldg(A + r * lda + a_col0 + c + i) : 0.f;
-              v0 = make_float4(t[0], t[1], t[2], t[3]);
-              v1 = make_float4(t[4], t[5], t[6], t[7]);
-            }
-          } else {
-            const float4* src = reinterpret_cast<const float4*>(B + r * ldb + 8 * grp);
+  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+  fence_regs(acc);
+
+  // a warp instruction covers 8 rows x 4 column groups of 8: lane = 8 * group + row, so a quarter-warp
+  // stores 8 consecutive rows of one column group (128 contiguous bytes of shared memory) and the four
+  // quarter-warps read one 128-byte piece of each of the 8 rows
+  const int lr = lane & 7, lg = lane >> 3;
+  for (int64_t it = 0; it < n_stage; ++it) {
+    const int s = (int)(it % kStages);
+    unsigned char* st = smem + s * kStageBytes;
+    unsigned char* a_hi = st;
+    unsigned char* a_lo = st + kABytes;
+    unsigned char* b_hi = st + 2 * kABytes;
+    unsigned char* b_lo = st + 2 * kABytes + kBBytes;
+    const int64_t r0 = r_begin + it * kStageRows;
+    // units: A has 8 row blocks x 4 group blocks (of 4 groups), B has 8 x 8; 96 units over 8 warps
+    for (int u = warp; u < 96; u += kWarps) {
+      const bool isA = u < 32;
+      const int uu = isA ? u : u - 32;
+      const int rb = uu & 7, gb = uu >> 3;
+      const int row = 8 * rb + lr;            // row within the stage = K index
+      const int grp = 4 * gb + lg;            // column group of 8 = MN index / 8
+      const int64_t r = r0 + row;
+      float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
+      if (r < r_end) {
+        if (isA) {
+          const int c = 8 * grp;
+          if (c + 8 <= ka && ((lda | a_col0) & 3) == 0) {
+            const float4* src = reinterpret_cast<const float4*>(A + r * lda + a_col0 + c);
             v0 = __ldg(src);
             v1 = __ldg(src + 1);
+          } else if (c < ka) {  // ragged edge / unaligned rows (k_in = 60, 87; the 2- and 4-column heads)
+            float t[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) t[i] = (c + i < ka) ? __ldg(A + r * lda + a_col0 + c + i) : 0.f;
+            v0 = make_float4(t[0], t[1], t[2], t[3]);
+            v1 = make_float4(t[4], t[5], t[6], t[7]);
           }
+        } else {
+          const float4* src = reinterpret_cast<const float4*>(B + r * ldb + 8 * grp);
+          v0 = __ldg(src);
+          v1 = __ldg(src + 1);
         }
-        uint4 hi, lo;
-        split8(v0, v1, hi, lo);
-        const uint32_t off = (uint32_t)(grp * (kStageRows * 16) + row * 16);
-        *reinterpret_cast<uint4*>((isA ? a_hi : b_hi) + off) = hi;
-        *reinterpret_cast<uint4*>((isA ? a_lo : b_lo) + off) = lo;
       }
-      fence_async_smem();  // own generic-proxy writes -> the tensor cores' async proxy, then the own arrival
-      mbar_arrive(&bars->full[s]);
+      uint4 hi, lo;
+      split8(v0, v1, hi, lo);
+      const uint32_t off = (uint32_t)(grp * (kStageRows * 16) + row * 16);
+      *reinterpret_cast<uint4*>((isA ? a_hi : b_hi) + off) = hi;
+      *reinterpret_cast<uint4*>((isA ? a_lo : b_lo) + off) = lo;
     }
-  } else {
-    // ---------------- MMA issue (one thread) -------------------------------------------------------
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(kTileM, kTileN, 1, 1);  // both operands MN-major
-      for (int64_t it = 0; it < n_stage; ++it) {
-        const int s = (int)(it % kStages);
-        mbar_wait(&bars->full[s], (uint32_t)((it / kStages) & 1));
-        tc_fence_after();
-        const uint32_t st = smem_u32(smem + s * kStageBytes);
-        // MN-major, no swizzle: 8-row (K) groups 128 bytes apart, 8-column (MN) groups kStageRows * 16 bytes apart
-        const uint64_t da_hi = make_desc(st, 128, kStageRows * 16), da_lo = make_desc(st + kABytes, 128, kStageRows * 16);
-        const uint64_t db_hi = make_desc(st + 2 * kABytes, 128, kStageRows * 16);
-        const uint64_t db_lo = make_desc(st + 2 * kABytes + kBBytes, 128, kStageRows * 16);
+    fence_async_smem();  // own generic-proxy writes -> the tensor cores' async proxy
+    wgmma_wait<0>();     // this warpgroup's MMAs of the previous stage are done (the other buffer is free
+    fence_regs(acc);     // once every warpgroup has passed the barrier below)
+    __syncthreads();
+    // MN-major, no swizzle: 8-row (K) groups 128 bytes apart, 8-column (MN) groups kStageRows * 16 bytes apart
+    const uint32_t sa = smem_u32(st) + (uint32_t)wg * 8 * (kStageRows * 16);  // this warpgroup's 64 columns of A
+    const uint32_t sb = smem_u32(st) + 2 * kABytes;
+    wgmma_fence();
 #pragma unroll
-        for (int ks = 0; ks < kStageRows / 16; ++ks) {
-          mma_f16(tmem, da_hi + 16 * ks, db_hi + 16 * ks, idesc, (it | ks) > 0);
-          mma_f16(tmem, da_lo + 16 * ks, db_hi + 16 * ks, idesc, 1);
-          mma_f16(tmem, da_hi + 16 * ks, db_lo + 16 * ks, idesc, 1);
-        }
-        mma_commit(&bars->empty[s]);
-      }
-      mma_commit(&bars->done);
+    for (int ks = 0; ks < kStageRows / 16; ++ks) {
+      const uint64_t da_hi = make_desc(sa + 256 * ks, 128, kStageRows * 16), da_lo = make_desc(sa + kABytes + 256 * ks, 128, kStageRows * 16);
+      const uint64_t db_hi = make_desc(sb + 256 * ks, 128, kStageRows * 16), db_lo = make_desc(sb + kBBytes + 256 * ks, 128, kStageRows * 16);
+      wgmma_n256<1, 1>(acc, da_hi, db_hi, 1);
+      wgmma_n256<1, 1>(acc, da_lo, db_hi, 1);
+      wgmma_n256<1, 1>(acc, da_hi, db_lo, 1);
     }
+    wgmma_commit();
   }
+  wgmma_wait<0>();
+  fence_regs(acc);
   // ---------------- epilogue: accumulator -> this slab's partial [128][256] -------------------------
-  if (n_stage > 0 && warp < 4) {
-    mbar_wait(&bars->done, 0);
-    tc_fence_after();
-    float* dst = partial + ((size_t)blockIdx.x * kTileM + 32 * warp + lane) * kTileN;
-    for (int cb = 0; cb < kTileN / 16; ++cb) {
-      float v[16];
-      tmem_ld16(tmem + ((uint32_t)(32 * warp) << 16) + cb * 16, v);
+  const int m0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+  float* dst = partial + ((size_t)blockIdx.x * kTileM) * kTileN;
 #pragma unroll
-      for (int i = 0; i < 4; ++i) reinterpret_cast<float4*>(dst + cb * 16)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-    }
-  } else if (n_stage == 0 && warp < 4) {
-    float* dst = partial + ((size_t)blockIdx.x * kTileM + 32 * warp + lane) * kTileN;
-    for (int c = 0; c < kTileN; ++c) dst[c] = 0.f;
+  for (int i = 0; i < 128; i += 2) {
+    const int m = m0 + 8 * ((i >> 1) & 1), n = 8 * (i >> 2) + 2 * (lane & 3);
+    *reinterpret_cast<float2*>(dst + (size_t)m * kTileN + n) = make_float2(acc[i], acc[i + 1]);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kProdWarps) tmem_dealloc(tmem, 256);
 }
 
 // partial[slab][m_rows][256] -> out[m][n] (row stride ld_out), slabs added in index order

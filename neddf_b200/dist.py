@@ -1,6 +1,6 @@
 """Multi-GPU rendering: rays shard over ranks, one all-gather of image tiles, nothing else.
 
-The reference is single-process (SURVEY 2: no torch.distributed anywhere); this is the B200
+The reference is single-process (SURVEY 2: no torch.distributed anywhere); this is the H100
 design of BASELINE.json north_star / SURVEY 8(e): one process per GPU, weights replicated
 (each rank loads the same 2.6 MB state_dict), the row-major pixel list of every frame is cut
 into ``world_size`` contiguous slices, each rank renders its slice with the single-GPU

@@ -1,4 +1,4 @@
-"""Make the reference's own scripts pick up the B200 renderer without editing them.
+"""Make the reference's own scripts pick up the CUDA renderer without editing them.
 
 ``neddf/scripts/run_eval.py`` re-composes the *saved* hydra config, whose ``_target_`` strings are
 always ``neddf.render.NeRFRender`` / ``neddf.network.NeDDF`` (SURVEY 8(b)).  Hydra resolves

@@ -1,5 +1,5 @@
 """python -m neddf_b200.launch <reference script.py> [args...]: run a reference entry point
-(neddf/scripts/run.py, run_eval.py) with NeRFRender / NeDDF rebound to the B200 classes.
+(neddf/scripts/run.py, run_eval.py) with NeRFRender / NeDDF rebound to the CUDA classes.
 NEDDF_B200_PATCH_TRAINER=1 also swaps in the vectorised ground-truth gather (trainer_glue.py)."""
 import os
 import runpy

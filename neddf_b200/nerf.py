@@ -1,4 +1,4 @@
-"""Drop-in for neddf.network.NeRF (neddf/network/nerf.py:13-178) on the B200 path: same constructor, same
+"""Drop-in for neddf.network.NeRF (neddf/network/nerf.py:13-178) on the CUDA path: same constructor, same
 module / state_dict layout (``layers.N``, ``outL_density``, ``outL_color.0`` / ``.2``), ``forward(Sampling)`` and
 ``set_iter``; the network itself runs in one CUDA kernel (``csrc/nerf_simt.cu`` behind ``neddf_nerf_*``).
 
@@ -289,7 +289,7 @@ class NeRF(BaseNeuralField):
             return False
         if not self.training_kernels:
             raise NotImplementedError(
-                "neddf_b200.NeRF is forward-only on the B200 path by default: wrap the call in torch.no_grad() / use "
+                "neddf_b200.NeRF is forward-only on the CUDA path by default: wrap the call in torch.no_grad() / use "
                 "render_image, or train with the reference and load the checkpoint.  The training backward kernel "
                 "(csrc/nerf_train.cu) is opt-in - net.training_kernels = True or NEDDF_NERF_TRAIN=1 - until it has been "
                 "run on hardware (so far: host emulation against the reference's autograd gradients)")

@@ -1,4 +1,4 @@
-"""Drop-in for neddf.network.NeuS (neddf/network/neus.py:12-162) on the B200 path: same constructor, same module /
+"""Drop-in for neddf.network.NeuS (neddf/network/neus.py:12-162) on the CUDA path: same constructor, same module /
 state_dict layout (``layers_sdf.N``, ``layers_col.N``, ``variance``) and ``forward(Sampling)``; the network runs in
 one CUDA kernel (``csrc/neus_simt.cu`` behind ``neddf_neus_*``).
 
@@ -140,7 +140,7 @@ class NeuS(BaseNeuralField):
     def _refuse_autograd(self) -> None:
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             raise NotImplementedError(
-                "neddf_b200.NeuS is forward-only on the B200 path (no backward kernel for this variant): wrap the call "
+                "neddf_b200.NeuS is forward-only on the CUDA path (no backward kernel for this variant): wrap the call "
                 "in torch.no_grad() / use render_image, or train with the reference and load the checkpoint")
 
     @staticmethod

@@ -301,7 +301,7 @@ class NeRFRender(BaseNeuralRender):
         self.network_fine.set_iter(iter)
 
     def set_engine(self, engine: str) -> None:
-        """"auto" | "fp32" (CUDA-core fp32 FMA) | "tc" (tcgen05, split-fp16 operands)."""
+        """"auto" | "fp32" (CUDA-core fp32 FMA) | "tc" (wgmma, split-fp16 operands) | "tc2" (the same kernel in CTA pairs)."""
         if engine not in L.ENGINE_IDS:
             raise ValueError(engine)
         for net in (self.network_fine, self.network_coarse):

@@ -78,7 +78,7 @@ def test_reference_gradients_against_the_fp64_arbiter():
     produced in fp32 (golden case_train, 26 tensors, loss over both passes) against the oracle's fp64 autograd run of
     the same step: the reference itself sits at ~2.4e-6 of the exact gradients, the fp32 restatement at the same
     distance and at 6e-7 of the reference.  The CUDA training path is measured at 1.6e-6 .. 3.5e-5 of fp64
-    (tools/grad_err.py, profiles/r02_summary.md section 5) - inside the 1e-4 the GPU tests assert
+    (tools/grad_err.py) - inside the 1e-4 the GPU tests assert
     (test_field_backward_matches_autograd; 2e-4 end to end through the resampling)."""
     c = Case("train")
 

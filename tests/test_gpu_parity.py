@@ -24,7 +24,7 @@ def _gpu():
 
 @pytest.mark.parametrize("n,k", [(128, 16), (128, 64), (128, 128), (16, 16), (16, 256)])
 def test_tc_selftest_gemm(n, k):
-    """tcgen05 building block (descriptor layouts, fp16-split 3-product accumulation) against an
+    """wgmma building block (descriptor layouts, fp16-split 3-product accumulation) against an
     fp64 GEMM: hidden configuration (n=128) and head configuration (n=16)."""
     G = _gpu()
     from neddf_b200 import _lib as L
@@ -336,7 +336,7 @@ def test_partition_of_unity_and_sorted_samples_at_full_chunk():
 
 
 def test_engines_agree_on_bench_workload():
-    """tcgen05 engine vs the fp32 FMA engine (device oracle) on 2,048 rays of the bench frame."""
+    """Tensor-core engines vs the fp32 FMA engine (device oracle) on 2,048 rays of the bench frame."""
     import bench
     G = _gpu()
     r_32, cam = _bench_render("fp32")
@@ -613,9 +613,9 @@ def test_network_forward_sampling_is_differentiable():
 
 
 def test_other_embedding_ranks_run_on_a_tensor_core_engine():
-    """The reference's own test fixture uses embed_pos_rank=6 (tests/conftest.py:77-99); the single-CTA
-    tensor-core kernel is built for ranks 10/4 only, the CTA-pair kernel covers any ranks that fit AUX:
-    "auto" must not fall to the 9x slower fp32 engine, and the result must match the oracle."""
+    """The reference's own test fixture uses embed_pos_rank=6 (tests/conftest.py:77-99); both tensor-core engines cover
+    any ranks whose inputs fit AUX: "auto" must not fall to the slower fp32 engine, and the results of "auto" (the
+    single-CTA engine) and of the CTA-pair engine must match the oracle."""
     G = _gpu()
     import neddf_b200
     cfg = dict(embed_pos_rank=6, embed_dir_rank=2, ddf_layer_count=5, col_layer_count=3, skips=[1],
@@ -626,7 +626,7 @@ def test_other_embedding_ranks_run_on_a_tensor_core_engine():
     net.load_state_dict(P)
     net.to(G.DEV)
     net.set_iter(-1)
-    assert net.resolved_engine() == "tc2"
+    assert net.resolved_engine() == "tc"
     g = torch.Generator().manual_seed(3)
     B, S = 5, 37
     pos = (torch.rand(B, S, 3, generator=g) - 0.5) * 2.0
@@ -635,10 +635,13 @@ def test_other_embedding_ranks_run_on_a_tensor_core_engine():
     st = orc.FieldState.at_iter(fc, -1)
     with torch.no_grad():
         ref = orc.field_forward(P, fc, st, pos, dd, var)
-        out = net(neddf_b200.Sampling(pos.to(G.DEV), dd.to(G.DEV), var.to(G.DEV)))
-    for k in ("distance", "density", "color", "fields_penalty", "aux_grad"):
-        assert nerr(out[k].cpu().numpy(), ref[k].numpy()) < PARITY_TOL, k
-    net.check_engine_status()
+    for engine in ("auto", "tc2"):
+        net.engine = engine
+        with torch.no_grad():
+            out = net(neddf_b200.Sampling(pos.to(G.DEV), dd.to(G.DEV), var.to(G.DEV)))
+        for k in ("distance", "density", "color", "fields_penalty", "aux_grad"):
+            assert nerr(out[k].cpu().numpy(), ref[k].numpy()) < PARITY_TOL, (engine, k)
+        net.check_engine_status()
 
 
 @pytest.mark.parametrize("engine", ["tc", "tc2", "fp32"])
@@ -720,7 +723,7 @@ def test_terminate_rays_kernel():
 @pytest.mark.parametrize("rows,lda,col0,ka", [(4096, 256, 0, 128), (100003, 256, 128, 128), (7777, 60, 0, 60), (5000, 87, 0, 87),
                                               (9001, 2, 0, 2), (6000, 4, 0, 3)])
 def test_wgrad_gemm(rows, lda, col0, ka):
-    """neddf_wgrad (tcgen05 split-K GEMM, fp16 hi/lo operands split on the fly) against an fp64 matmul:
+    """neddf_wgrad (wgmma split-K GEMM, fp16 hi/lo operands split on the fly) against an fp64 matmul:
     the shapes of the training backward (aligned / ragged / 2- and 3-column head operands, slab remainders)."""
     G = _gpu()
     from neddf_b200 import _lib as L
@@ -851,48 +854,44 @@ def test_sample_pdf_without_coarse_edges():
 
 @pytest.mark.parametrize("case,n_rays", [("bunny", 1), ("bunny", 3), ("bunny", 37), ("bunny", 600), ("bunny", 2500),
                                          ("default", 600), ("point", 600), ("leaky", 600)])
-def test_tc_batched_colour_trunk_matches_per_tile_program(case, n_rays, monkeypatch):
-    """Images-only launches of the tc engine run the colour trunk once per group of four tiles
-    (TcParams::batch, DESIGN 4.1).  Same results as the per-tile program (NEDDF_TC_BATCH=1) for launches
-    with fewer tiles than CTAs, ragged last tiles and groups of 1, 2, 3 and 4 tiles per CTA, for every golden
-    configuration (activations, skips, sampling types), and as the oracle (neddf.py:200-257 through
-    oracle.field_forward)."""
+def test_tc_images_only_colour_trunk_matches_full_program(case, n_rays):
+    """Images-only launches of the tc engine (no fields_penalty) run the colour trunk on the 32 value rows of a tile
+    (N = 32 MMAs, DESIGN 4.1).  Same results as the full program (N = 128, Jacobian rows included) for launches with
+    fewer tiles than CTAs, ragged last tiles and several tiles per CTA, for every golden configuration (activations,
+    skips, sampling types), and as the oracle (neddf.py:200-257 through oracle.field_forward)."""
     import neddf_b200
     G = _gpu()
     c = Case(case)
     render = G.build_render(c, "tc")
     net = render.network_fine
-    if net.resolved_engine(G.DEV) != "tc":
-        pytest.skip("this configuration does not run on the tc engine")
+    assert net.resolved_engine(G.DEV) == "tc"
     g = torch.Generator().manual_seed(n_rays)
     uv = torch.stack([torch.randint(0, 50, (n_rays,), generator=g), torch.randint(0, 50, (n_rays,), generator=g)], 1).float()
     d, o = orc.make_rays(uv, c.cam)
     dists = orc.coarse_dists(c.rc, torch.rand(n_rays, c.rc.sample_coarse + 1, generator=g))
     radius = neddf_b200.ray.CONE_RAY_RADIUS if c.rc.sampling_type == "cone" else 0.0
 
-    def run():
+    def run(need_penalty):
         with torch.no_grad():
             out = net.forward_rays(d.to(G.DEV), o.to(G.DEV), dists.to(G.DEV), c.rc.sampling_type, radius,
-                                   need_penalty=False, need_aux=True)
+                                   need_penalty=need_penalty, need_aux=True)
         torch.cuda.synchronize()
         net.check_engine_status()
         return {k: v.cpu() for k, v in out.items()}
 
-    batched = run()
-    monkeypatch.setenv("NEDDF_TC_BATCH", "1")
-    per_tile = run()
-    monkeypatch.delenv("NEDDF_TC_BATCH")
+    images = run(False)
+    full = run(True)
     for k in ("density", "distance", "aux_grad"):
-        assert torch.equal(batched[k], per_tile[k]), k  # the distance trunk is the same program
-    # colour: N = 128 instead of N = 32 MMAs over the same operands
-    assert nerr(batched["color"].numpy(), per_tile["color"].numpy()) < 1e-6
+        assert torch.equal(images[k], full[k]), k  # the distance trunk is the same program
+    # colour: N = 32 instead of N = 128 MMAs over the same value rows
+    assert nerr(images["color"].numpy(), full["color"].numpy()) < 1e-6
     pos, dd, var = orc.make_samples(c.rc, d, o, dists)
     with torch.no_grad():
         ref = orc.field_forward(c.p_fine, c.fc, c.st, pos, dd, var)
     # (random pixels mostly look past the bunny: densities of 1e-2 and below, for which max|ref| is no scale -
     # the floor of 1 keeps the bound absolute there; colours are O(1))
     for k in ("density", "color"):
-        a, r = batched[k].numpy(), ref[k].numpy()
+        a, r = images[k].numpy(), ref[k].numpy()
         e = np.abs(a.astype(np.float64) - r) / max(np.abs(r).max(), 1.0)
         if c.kinked:  # same allowance as helpers.assert_parity: the few samples within rounding distance of a kink
             assert int((e >= PARITY_TOL).sum()) <= max(2, int(1e-2 * e.size)) and e.max() < 5e-2, (k, e.max())

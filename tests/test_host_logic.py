@@ -71,17 +71,19 @@ def test_neus_module_surface_matches_the_reference():
     for n, cin, cout in shapes:  # torch nn.Linear keeps [out, in]
         assert tuple(sd[n + ".weight"].shape) == (cout, cin) and tuple(sd[n + ".bias"].shape) == (cout,)
     assert abs(float(sd["variance"]) - 0.45) < 1e-7
-    ref_root = "/root/reference"
-    if os.path.isdir(ref_root):
-        sys.path.insert(0, ref_root)
-        try:
-            from neddf.network import NeuS as RefNeuS
-            torch.manual_seed(7)
-            ref = RefNeuS(**kw).state_dict()
-        finally:
-            sys.path.remove(ref_root)
-        assert list(ref) == list(sd)
-        assert all(torch.equal(ref[k], sd[k]) for k in ref)
+    # the reference's NeuS(**kw) after the same seed, recorded by tests/golden/make_host_golden.py
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
+    try:
+        from make_host_golden import NEUS_KW, neus_fingerprint
+    finally:
+        sys.path.pop(0)
+    assert kw == NEUS_KW
+    z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "case_neus_init.npz"))
+    fk, fshapes, fsums, fsamples = neus_fingerprint(sd)
+    assert fk == list(z["keys"])
+    assert np.array_equal(fshapes, z["shapes"])
+    assert np.array_equal(fsamples, z["samples"])
+    assert np.allclose(fsums, z["sums"], rtol=1e-12, atol=1e-12)
     r = neddf_b200.NeRFRender(network_config={"_target_": "neddf.network.NeuS", **kw}, use_coarse_network=False)
     assert isinstance(r.network_fine, neddf_b200.NeuS) and r.network_coarse is r.network_fine
     assert len(r.get_parameters_list()) == 2 * len(shapes) + 1
@@ -111,24 +113,35 @@ def test_camera_standin_matches_reference_pose():
     assert np.allclose(cam2.T.numpy(), [1, 2, 3])
 
 
-@pytest.mark.skipif(not __import__("os").path.isdir("/root/reference/neddf"), reason="reference tree not present")
 def test_install_rebinds_reference_targets(repo_root):
-    """neddf_b200.install makes the saved `_target_` strings resolve to the B200 classes and the
-    pretrained checkpoint loads unchanged (subprocess: do not pollute this interpreter's modules)."""
+    """neddf_b200.install makes the saved `_target_` strings of the reference's pretrained bunny_smoke run resolve to
+    the CUDA classes, their state_dict has the keys and shapes of the run's checkpoint, and the recorded weights of
+    that checkpoint load unchanged.  The config nodes and the checkpoint's keys / shapes / sums are recorded from the
+    reference (tests/golden/case_bunny_checkpoint.npz, tests/golden/make_host_golden.py); the reference's
+    `neddf.render` / `neddf.network` packages are stand-in modules (subprocess: do not pollute this interpreter)."""
     import os
     import subprocess
     import sys
     code = (
-        "import sys, yaml, torch, hydra\n"
-        "import neddf_b200.install as I; I.install()\n"
-        "cfg = yaml.safe_load(open('/root/reference/pretrained/bunny_smoke/.hydra/config.yaml'))\n"
-        "r = hydra.utils.instantiate(dict(cfg['render']), network_config=cfg['network'])\n"
+        "import json, sys, types, numpy as np, torch\n"
+        "for n in ('neddf', 'neddf.render', 'neddf.render.nerf_render', 'neddf.network', 'neddf.network.neddf'):\n"
+        "    sys.modules[n] = types.ModuleType(n)\n"
+        "import hydra, neddf_b200.install as I; I.install()\n"
+        "from tests.golden.make_host_golden import neus_fingerprint\n"
+        "from tests.helpers import Case\n"
+        "z = np.load('tests/golden/case_bunny_checkpoint.npz')\n"
+        "r = hydra.utils.instantiate(json.loads(str(z['render'])), network_config=json.loads(str(z['network'])))\n"
         "assert type(r).__module__ == 'neddf_b200.render' and type(r.network_fine).__module__ == 'neddf_b200.network'\n"
-        "res = r.load_state_dict(torch.load('/root/reference/pretrained/bunny_smoke/models/model_02000.pth', map_location='cpu'))\n"
+        "keys, shapes, _, _ = neus_fingerprint(r.state_dict())\n"
+        "assert keys == list(z['keys']) and np.array_equal(shapes, z['shapes'])\n"
+        "sd = Case('bunny').state_dict()\n"
+        "res = r.load_state_dict(sd)\n"
         "assert not res.missing_keys and not res.unexpected_keys\n"
+        "_, _, sums, _ = neus_fingerprint(r.state_dict())\n"
+        "assert np.allclose(sums, z['sums'], rtol=1e-6, atol=1e-6)  # the recorded weights are the checkpoint's\n"
         "print('ok')\n")
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join(["/root/reference", os.path.join(repo_root, "tests/golden/_refstub"), repo_root]))
-    out = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=300)
+    env = dict(os.environ, PYTHONPATH=os.pathsep.join([os.path.join(repo_root, "tests/golden/_refstub"), repo_root]))
+    out = subprocess.run([sys.executable, "-c", code], cwd=repo_root, env=env, capture_output=True, text=True, timeout=300)
     assert out.returncode == 0 and "ok" in out.stdout, out.stderr[-2000:]
 
 
@@ -163,33 +176,44 @@ def test_vectorised_ground_truth_gather_is_bit_exact():
     assert gather_targets(item, us[:0], vs[:0], ["ColorLoss"], "cpu")["color"].shape == (0, 3)
 
 
-@pytest.mark.skipif(not __import__("os").path.isdir("/root/reference/neddf"), reason="reference tree not present")
 def test_trainer_patch_matches_reference_method(repo_root):
-    """install(patch_trainer=True) swaps BaseTrainer.construct_ground_truth for the vectorised gather;
-    the reference's own method gives the same tensors (subprocess; skimage/hydra stubbed)."""
+    """install(patch_trainer=True) swaps BaseTrainer.construct_ground_truth for the vectorised gather (checked in a
+    subprocess on a stand-in of the reference's trainer module); the reference's own method gave the same tensors
+    on the recorded inputs (tests/golden/case_trainer_gather.npz, tests/golden/make_host_golden.py)."""
     import os
     import subprocess
     import sys
+
+    from neddf_b200.trainer_glue import construct_ground_truth
+    z = np.load(os.path.join(repo_root, "tests", "golden", "case_trainer_gather.npz"))
+
+    class T:
+        pass
+
+    t = T()
+    t.device = torch.device("cpu")
+    t.dataset = [dict(rgb_images=z["rgb"], mask_images=z["mask"])]
+    kinds = ["ColorLoss", "MaskBCELoss", "FieldsConstraintLoss"]
+    got = construct_ground_truth(t, 0, torch.from_numpy(z["us"]), torch.from_numpy(z["vs"]), kinds)
+    assert sorted(got) == list(z["keys"])
+    for k in got:
+        assert str(got[k].dtype) == str(z["dtype_" + k]) and np.array_equal(got[k].numpy(), z["out_" + k]), k
     code = (
-        "import sys, types, numpy as np, torch\n"
-        "sk = types.ModuleType('skimage'); m = types.ModuleType('skimage.metrics')\n"
-        "m.peak_signal_noise_ratio = m.structural_similarity = None; sk.metrics = m\n"
-        "sys.modules['skimage'] = sk; sys.modules['skimage.metrics'] = m\n"
-        "from neddf.trainer.base_trainer import BaseTrainer\n"
-        "ref_fn = BaseTrainer.construct_ground_truth\n"
-        "import neddf_b200.install as I; I.install(patch_trainer=True)\n"
-        "assert BaseTrainer.construct_ground_truth is not ref_fn\n"
-        "rng = np.random.default_rng(3)\n"
-        "class T: pass\n"
-        "t = T(); t.device = torch.device('cpu')\n"
-        "t.dataset = [dict(rgb_images=rng.integers(0, 256, (20, 30, 3), dtype=np.uint8), mask_images=rng.integers(0, 256, (20, 30), dtype=np.uint8))]\n"
-        "us = (torch.rand(64) * 29).to(torch.int16); vs = (torch.rand(64) * 19).to(torch.int16)\n"
-        "kinds = ['ColorLoss', 'MaskBCELoss', 'FieldsConstraintLoss']\n"
-        "a = ref_fn(t, 0, us, vs, kinds); b = BaseTrainer.construct_ground_truth(t, 0, us, vs, kinds)\n"
-        "assert set(a) == set(b) and all(torch.equal(a[k], b[k]) and a[k].dtype == b[k].dtype for k in a)\n"
+        "import sys, types\n"
+        "mods = {n: types.ModuleType(n) for n in ('neddf', 'neddf.render', 'neddf.network', 'neddf.trainer',\n"
+        "                                          'neddf.trainer.base_trainer', 'neddf.loss')}\n"
+        "class BaseTrainer:\n"
+        "    def construct_ground_truth(self, *a): raise AssertionError('reference method still bound')\n"
+        "mods['neddf.trainer.base_trainer'].BaseTrainer = BaseTrainer\n"
+        "sys.modules.update(mods)\n"
+        "import neddf_b200, neddf_b200.install as I, neddf_b200.trainer_glue as G, neddf_b200.losses as Lo\n"
+        "I.install(patch_trainer=True)\n"
+        "assert BaseTrainer.construct_ground_truth is G.construct_ground_truth\n"
+        "assert mods['neddf.render'].NeRFRender is neddf_b200.NeRFRender and mods['neddf.network'].NeDDF is neddf_b200.NeDDF\n"
+        "assert all(getattr(mods['neddf.loss'], n) is getattr(Lo, n) for n in ('ColorLoss', 'MaskBCELoss', 'FieldsConstraintLoss'))\n"
         "print('ok')\n")
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join(["/root/reference", os.path.join(repo_root, "tests/golden/_refstub"), repo_root]))
-    out = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=300)
+    out = subprocess.run([sys.executable, "-c", code], cwd=repo_root, env=dict(os.environ, PYTHONPATH=repo_root),
+                         capture_output=True, text=True, timeout=300)
     assert out.returncode == 0 and "ok" in out.stdout, out.stderr[-2000:]
 
 

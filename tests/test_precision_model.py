@@ -65,7 +65,7 @@ def test_bf16_parts_cost_an_order_of_magnitude():
 def test_fp8_lo_weights_keep_the_bar_but_not_the_margin():
     """lo parts of the weights as e4m3 * 2^S (25 % fewer weight bytes): inside 1e-4 on smooth
     configurations but 5-20x worse than fp16 lo parts; on hardware it was no faster and broke the
-    kinked (ReLU / point-sampling) case - rejected (profiles/r01_summary.md)."""
+    kinked (ReLU / point-sampling) case - rejected."""
     cfg, P, *_ = _case()
     maxlo = max(float((v - _h(v)).abs().max()) for k, v in P.items() if k.endswith("weight"))
     S = min(24, math.floor(math.log2(240 / maxlo)))
