@@ -434,6 +434,45 @@ int32_t neddf_nerf_train_backward_rays(const neddf_nerf_train_t* h, const float*
                                        float* d_x, float* d_g, float* d_e, float* d_d, float* d_c1, float* d_gc1, float* d_gzd,
                                        void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * NeuS field variant, training backward: the autograd graph of NeuS.forward (neus.py:101-162) with respect to the
+ * parameters nerf_trainer.py:38-42 hands to Adam (every Linear and `variance`), second order through the normal that
+ * neus.py:133-142 takes with torch.autograd.grad(create_graph=True).  fp32 CUDA-core kernel (csrc/neus_train.cu +
+ * csrc/neus_train_kernel.cuh): one launch recomputes the forward per 64-sample tile, walks back through the colour and
+ * SDF trunks and leaves the operands of the weight-gradient GEMMs in global memory; the gradients themselves are
+ * neddf_wgrad / neddf_colsum_value_rows calls on those buffers (what neddf_b200/neus.py does).
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct neddf_neus_train neddf_neus_train_t; /* opaque: config + forward and transposed weight packs */
+
+/* NeuS.__init__ (neus.py:29-99); same configurations as neddf_neus_create. */
+int32_t neddf_neus_train_create(const neddf_neus_config_t* cfg, neddf_neus_train_t** out);
+void neddf_neus_train_destroy(neddf_neus_train_t* h);
+/* Same arguments as neddf_neus_set_weights (layers_sdf.*, layers_col.*, variance: neus.py:83-99). */
+int32_t neddf_neus_train_set_weights(neddf_neus_train_t* h, const float* const* d_w, const float* const* d_b, int32_t n_layers,
+                                     const float* d_variance, void* stream);
+
+/* Backward of NeuS.forward (neus.py:101-162) on n explicit samples.  Upstream gradients: d_g_sdf [n] (NULL = none),
+ * d_g_density [n], d_g_color [n,3], d_g_normal [n,3] (NULL = none).  d_bufs = nine fp32 outputs, the sample as the row
+ * (Ls = sdf_layer_count, Lc = col_layer_count, n_e = 6 embed_pos_rank, n_x = 6 + 6 embed_dir_rank):
+ *   [0] E4  [n][4][n_e]       position embedding + its Jacobian rows     [1] XS [Ls-1][n][4][256] SDF layer outputs (y, J_y)
+ *   [2] GS  [Ls][n][4][256]   SDF pre-activation gradients (g_z, g_Jz)   [3] XC0 [n][n_x] [pos | dir PE | normal]
+ *   [4] FO  [n][256]          trunk features                             [5] XC [Lc][n][256] colour activations
+ *   [6] GC  [Lc][n][256]      colour pre-activation gradients            [7] GH [n][3] head pre-activation gradient
+ *   [8] GV  [n]               d loss / d variance per sample
+ * Then, with in_0 = E4, in_l = [XS_{l-1} | E4 if l-1 in skips] over the 4 n rows:
+ *   d layers_sdf.l.weight^T = in_l^T GS_l, d layers_sdf.l.bias = sum of the value rows of GS_l,
+ *   d layers_col.0.weight^T = [XC0 | FO]^T GC_0, d layers_col.l.weight^T = XC_{l-1}^T GC_l, d bias = colsum GC_l,
+ *   d layers_col.Lc.weight = GH^T XC_{Lc-1}, d bias = colsum GH, d variance = sum GV. */
+int32_t neddf_neus_train_backward(const neddf_neus_train_t* h, const float* d_pos, const float* d_dir, int64_t n,
+                                  const float* d_g_sdf, const float* d_g_density, const float* d_g_color, const float* d_g_normal,
+                                  float* const* d_bufs, void* stream);
+/* Same with the sample geometry fused (rays [n_rays,3], dists [n_rays, n_edges]; n = n_rays * n_edges), as
+ * neddf_neus_forward_rays (nerf_render.py:123-147). */
+int32_t neddf_neus_train_backward_rays(const neddf_neus_train_t* h, const float* d_ray_dir, const float* d_ray_orig,
+                                       const float* d_dists, int64_t n_rays, int32_t n_edges, int32_t sampling_type,
+                                       float ray_radius, const float* d_g_sdf, const float* d_g_density, const float* d_g_color,
+                                       const float* d_g_normal, float* const* d_bufs, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

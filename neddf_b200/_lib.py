@@ -116,6 +116,11 @@ _SIGNATURES = {
     "neddf_neus_set_weights": (_I32, [_P, C.POINTER(_P), C.POINTER(_P), _I32, _P, _P]),
     "neddf_neus_forward": (_I32, [_P, _P, _P, _I64, _P, _P, _P, _P, _P]),
     "neddf_neus_forward_rays": (_I32, [_P, _P, _P, _P, _I64, _I32, _I32, _F, _P, _P, _P, _P, _P]),
+    "neddf_neus_train_create": (_I32, [C.POINTER(NeusConfig), C.POINTER(_P)]),
+    "neddf_neus_train_destroy": (None, [_P]),
+    "neddf_neus_train_set_weights": (_I32, [_P, C.POINTER(_P), C.POINTER(_P), _I32, _P, _P]),
+    "neddf_neus_train_backward": (_I32, [_P, _P, _P, _I64, _P, _P, _P, _P, C.POINTER(_P), _P]),
+    "neddf_neus_train_backward_rays": (_I32, [_P, _P, _P, _P, _I64, _I32, _I32, _F, _P, _P, _P, _P, C.POINTER(_P), _P]),
 }
 
 _lib = None

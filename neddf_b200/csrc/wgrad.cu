@@ -17,6 +17,12 @@
 // in 128 fp32 registers per thread.  The slab's partial result goes to a workspace and a second kernel adds
 // the slabs in a fixed order (deterministic gradients, no atomics).
 //
+// fp16 has a narrow exponent range: gradients of a loss averaged over many rays sit around 1e-5 .. 1e-8, where the hi
+// part is subnormal (absolute precision 6e-8) and the lo part underflows - the products then lose up to a few 1e-3 of
+// their value.  So every column of A and of B is first scaled by a power of two that puts its largest magnitude at
+// 2^14 (col_absmax_kernel + atomicMax on the bit patterns, order-independent), and the reducer divides the scales
+// out again; powers of two are exact, so the result is the product of the unscaled operands to the same rounding.
+//
 // The bias gradient (sum of gy over the value rows) is a column sum: colsum_rows_kernel + the same reducer.
 #include "tc_ptx.cuh"
 
@@ -36,7 +42,35 @@ constexpr uint32_t kBBytes = kTileN * kStageRows * 2;  // 32 KB per hi / lo
 constexpr uint32_t kStageBytes = 2 * kABytes + 2 * kBBytes;  // 96 KB
 constexpr int kWarps = 8;
 constexpr int kThreads = kWarps * 32;
-constexpr uint32_t kSmemBytes = kStages * kStageBytes;
+constexpr uint32_t kScaleOff = kStages * kStageBytes;                  // [128 + 256] column scale factors
+constexpr uint32_t kSmemBytes = kScaleOff + (kTileM + kTileN) * sizeof(float);
+
+// exponent that puts a column whose largest magnitude has the bit pattern `bits` at [2^14, 2^15) (0 for an all-zero
+// or non-finite column)
+__device__ __forceinline__ int scale_exp(uint32_t bits) {
+  const float m = __uint_as_float(bits);
+  if (!(m > 0.f) || !isfinite(m)) return 0;
+  return max(-100, min(100, 14 - ilogbf(m)));
+}
+
+// amax[m] = max |A[r][a_col0 + m]|, bmax[n] = max |B[r][n]| over all rows, as float bit patterns (zeroed by the caller)
+__global__ void __launch_bounds__(kTileM + kTileN)
+    col_absmax_kernel(const float* __restrict__ A, int64_t lda, int a_col0, int ka, const float* __restrict__ B, int64_t ldb,
+                      int64_t rows, int64_t rows_per_block, uint32_t* __restrict__ amax, uint32_t* __restrict__ bmax) {
+  const int t = threadIdx.x;
+  const int64_t r0 = (int64_t)blockIdx.x * rows_per_block, r1 = min(rows, r0 + rows_per_block);
+  float m = 0.f;
+  if (t < kTileM) {
+    if (t < ka)
+#pragma unroll 8
+      for (int64_t r = r0; r < r1; ++r) m = fmaxf(m, fabsf(__ldg(A + r * lda + a_col0 + t)));
+    atomicMax(amax + t, __float_as_uint(m));
+  } else {
+#pragma unroll 8
+    for (int64_t r = r0; r < r1; ++r) m = fmaxf(m, fabsf(__ldg(B + r * ldb + (t - kTileM))));
+    atomicMax(bmax + (t - kTileM), __float_as_uint(m));
+  }
+}
 
 // 8 consecutive fp32 -> 8 fp16 hi (16 bytes) + 8 fp16 lo
 __device__ __forceinline__ void split8(const float4& a, const float4& b, uint4& hi, uint4& lo) {
@@ -59,9 +93,15 @@ __device__ __forceinline__ void split8(const float4& a, const float4& b, uint4& 
 //   B: [rows][ldb] fp32, 256 columns
 __global__ void __launch_bounds__(kThreads, 1)
     wgrad_gemm_kernel(const float* __restrict__ A, int64_t lda, int a_col0, int ka, const float* __restrict__ B, int64_t ldb,
-                      int64_t rows, int64_t rows_per_slab, float* __restrict__ partial) {
+                      int64_t rows, int64_t rows_per_slab, const uint32_t* __restrict__ amax, const uint32_t* __restrict__ bmax,
+                      float* __restrict__ partial) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
+  float* fa = reinterpret_cast<float*>(smem + kScaleOff);  // column scale factors of A (128) and B (256)
+  float* fb = fa + kTileM;
+  if (tid < kTileM) fa[tid] = ldexpf(1.f, scale_exp(amax[tid]));
+  fb[tid] = ldexpf(1.f, scale_exp(bmax[tid]));
+  __syncthreads();
   const int64_t r_begin = (int64_t)blockIdx.x * rows_per_slab;
   const int64_t r_end = min(rows, r_begin + rows_per_slab);
   const int64_t n_stage = (r_end > r_begin) ? (r_end - r_begin + kStageRows - 1) / kStageRows : 0;
@@ -112,6 +152,9 @@ __global__ void __launch_bounds__(kThreads, 1)
           v1 = __ldg(src + 1);
         }
       }
+      const float* f8 = (isA ? fa : fb) + 8 * grp;
+      v0 = make_float4(v0.x * f8[0], v0.y * f8[1], v0.z * f8[2], v0.w * f8[3]);
+      v1 = make_float4(v1.x * f8[4], v1.y * f8[5], v1.z * f8[6], v1.w * f8[7]);
       uint4 hi, lo;
       split8(v0, v1, hi, lo);
       const uint32_t off = (uint32_t)(grp * (kStageRows * 16) + row * 16);
@@ -148,14 +191,17 @@ __global__ void __launch_bounds__(kThreads, 1)
   }
 }
 
-// partial[slab][m_rows][256] -> out[m][n] (row stride ld_out), slabs added in index order
+// partial[slab][m_rows][256] -> out[m][n] (row stride ld_out), slabs added in index order, column scales (if any)
+// divided out
 __global__ void reduce_partials_kernel(const float* __restrict__ partial, int n_slabs, int tile_rows, int m_rows,
-                                       float* __restrict__ out, int64_t ld_out, int n_cols) {
+                                       float* __restrict__ out, int64_t ld_out, int n_cols, const uint32_t* __restrict__ amax,
+                                       const uint32_t* __restrict__ bmax) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= m_rows * kTileN) return;
   const int m = idx / kTileN, n = idx % kTileN;
   float acc = 0.f;
   for (int s = 0; s < n_slabs; ++s) acc += partial[((size_t)s * tile_rows + m) * kTileN + n];
+  if (amax) acc = ldexpf(acc, -(scale_exp(amax[m]) + scale_exp(bmax[n])));
   if (n < n_cols) out[(size_t)m * ld_out + n] = acc;
 }
 
@@ -181,7 +227,9 @@ __global__ void colsum_rows_kernel(const float* __restrict__ G, int64_t n_sample
 
 using namespace neddf;
 
-extern "C" int64_t neddf_wgrad_workspace_bytes(void) { return (int64_t)sm_count() * wg::kTileM * wg::kTileN * sizeof(float); }
+// slab partials, then the column maxima of A (128) and B (256)
+static int64_t partial_floats() { return (int64_t)sm_count() * wg::kTileM * wg::kTileN; }
+extern "C" int64_t neddf_wgrad_workspace_bytes(void) { return (partial_floats() + wg::kTileM + wg::kTileN) * (int64_t)sizeof(float); }
 
 extern "C" int32_t neddf_wgrad(const float* d_a, int64_t lda, int32_t a_col0, int32_t ka, const float* d_b, int64_t ldb,
                                int64_t rows, float* d_out, int64_t ld_out, int32_t n_cols, float* d_workspace, void* stream) {
@@ -195,11 +243,19 @@ extern "C" int32_t neddf_wgrad(const float* d_a, int64_t lda, int32_t a_col0, in
   int64_t per = (rows + n_slabs - 1) / n_slabs;
   per = (per + wg::kStageRows - 1) / wg::kStageRows * wg::kStageRows;
   n_slabs = (int)((rows + per - 1) / per);
+  uint32_t* amax = reinterpret_cast<uint32_t*>(d_workspace + partial_floats());
+  uint32_t* bmax = amax + wg::kTileM;
+  NEDDF_CUDA_CHECK(cudaMemsetAsync(amax, 0, (wg::kTileM + wg::kTileN) * sizeof(uint32_t), s));
+  const int max_blocks = (int)std::min<int64_t>(4 * sm_count(), (rows + 255) / 256);
+  const int64_t max_per = (rows + max_blocks - 1) / max_blocks;
+  wg::col_absmax_kernel<<<(int)((rows + max_per - 1) / max_per), wg::kTileM + wg::kTileN, 0, s>>>(d_a, lda, a_col0, ka, d_b, ldb, rows,
+                                                                                                  max_per, amax, bmax);
+  NEDDF_LAUNCH_CHECK();
   NEDDF_CUDA_CHECK(cudaFuncSetAttribute(wg::wgrad_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg::kSmemBytes));
-  wg::wgrad_gemm_kernel<<<n_slabs, wg::kThreads, wg::kSmemBytes, s>>>(d_a, lda, a_col0, ka, d_b, ldb, rows, per, d_workspace);
+  wg::wgrad_gemm_kernel<<<n_slabs, wg::kThreads, wg::kSmemBytes, s>>>(d_a, lda, a_col0, ka, d_b, ldb, rows, per, amax, bmax, d_workspace);
   NEDDF_LAUNCH_CHECK();
   const int total = ka * wg::kTileN;
-  wg::reduce_partials_kernel<<<(total + 255) / 256, 256, 0, s>>>(d_workspace, n_slabs, wg::kTileM, ka, d_out, ld_out, n_cols);
+  wg::reduce_partials_kernel<<<(total + 255) / 256, 256, 0, s>>>(d_workspace, n_slabs, wg::kTileM, ka, d_out, ld_out, n_cols, amax, bmax);
   NEDDF_LAUNCH_CHECK();
   return NEDDF_OK;
 }
@@ -214,7 +270,7 @@ extern "C" int32_t neddf_colsum_value_rows(const float* d_g, int64_t n_samples, 
   n_slabs = (int)((n_samples + per - 1) / per);
   wg::colsum_rows_kernel<<<n_slabs, wg::kTileN, 0, s>>>(d_g, n_samples, sample_stride, per, d_workspace);
   NEDDF_LAUNCH_CHECK();
-  wg::reduce_partials_kernel<<<1, 256, 0, s>>>(d_workspace, n_slabs, 1, 1, d_out, wg::kTileN, wg::kTileN);
+  wg::reduce_partials_kernel<<<1, 256, 0, s>>>(d_workspace, n_slabs, 1, 1, d_out, wg::kTileN, wg::kTileN, nullptr, nullptr);
   NEDDF_LAUNCH_CHECK();
   return NEDDF_OK;
 }

@@ -7,10 +7,16 @@ autograd enabled - its own ``render_image`` (grad disabled, nerf_render.py:218) 
 normal is carried forward through the SDF trunk inside the kernel, so ``forward`` / ``render_rays`` under
 ``torch.no_grad()`` and ``render_image`` work.
 
-Scope (SURVEY 8(f) item 3): inference.  There is no backward kernel for this variant: calling it with autograd
-enabled on trainable parameters raises (train with the reference, load the checkpoint here).  No CPU / PyTorch
-fallback."""
+Scope (SURVEY 8(f) item 3): inference.  By default a call with autograd enabled on trainable parameters raises.
+No CPU / PyTorch fallback.
+
+Training (opt-in: ``net.training_kernels = True`` or NEDDF_NEUS_TRAIN=1): the backward of the autograd graph of
+neus.py:101-162 with respect to the parameters - second order through the normal, which the reference takes with
+autograd.grad(create_graph=True) - runs in ``csrc/neus_train.cu`` (forward recomputed per tile, data gradients in fp32
+FMA) + ``neddf_wgrad`` / ``neddf_colsum_value_rows`` (weight / bias gradients).  ``forward`` / ``forward_rays`` then
+return tensors with a ``grad_fn`` and ``NeRFRender.render_rays`` trains through the compositing backward."""
 import ctypes as C
+import os
 from typing import Dict, List, Optional
 
 import torch
@@ -19,6 +25,105 @@ from torch import Tensor, nn
 from . import _lib as L
 from .network import BaseNeuralField
 from .ray import Sampling
+
+
+class _NeusTrainFn(torch.autograd.Function):
+    """NeuS.forward under autograd.  forward: the inference kernel (neddf_neus_forward[_rays]); backward:
+    neddf_neus_train_backward[_rays] (recomputes the forward per tile, leaves the layer inputs and pre-activation
+    gradients in global memory), then gW = X^T G as tensor-core split-K GEMMs (neddf_wgrad), bias gradients as column
+    sums of the value rows and d variance as the sum of the per-sample terms.  Gradients flow to the module's parameters
+    only (nerf_trainer.py:38-42 optimises nothing else)."""
+
+    @staticmethod
+    def forward(ctx, net, a, b, c, sampling_type, ray_radius, with_normal, *params):
+        """(a, b, c) = (ray_dir[B,3], ray_orig[B,3], dists[B,S]) with a sampling type, or (pos, dir)[B,S,3] and c = None
+        when sampling_type is None."""
+        with torch.no_grad():
+            out = net._launch_forward(a, b, c, sampling_type, ray_radius, with_normal)
+        ctx.net, ctx.meta = net, (sampling_type, float(ray_radius))
+        ctx.save_for_backward(a, b, c)
+        return (out["sdf"], out["density"], out["color"]) + ((out["normal"],) if with_normal else ())
+
+    @staticmethod
+    def backward(ctx, g_sdf, g_density, g_color, g_normal=None):
+        net = ctx.net
+        a, b, c = ctx.saved_tensors
+        sampling_type, ray_radius = ctx.meta
+        from_rays = sampling_type is not None
+        B, S = (c.shape if from_rays else a.shape[:2])
+        n = B * S
+        device = a.device
+        W, Ls, Lc = 256, net.sdf_layer_count, net.col_layer_count
+        n_e, n_x = 6 * net.embed_pos_rank, 6 + 6 * net.embed_dir_rank
+
+        def prep(g, shape, zero_fill):
+            if g is None:
+                return torch.zeros(shape, device=device, dtype=torch.float32) if zero_fill else None
+            return g.contiguous().to(torch.float32)
+
+        g_sdf, g_density = prep(g_sdf, (B, S), False), prep(g_density, (B, S), True)
+        g_color, g_normal = prep(g_color, (B, S, 3), True), prep(g_normal, (B, S, 3), False)
+        f32 = dict(device=device, dtype=torch.float32)
+        E4 = torch.empty(n, 4, n_e, **f32)
+        XS = torch.empty(max(Ls - 1, 1), n, 4, W, **f32)
+        GS = torch.empty(Ls, n, 4, W, **f32)
+        XC0 = torch.empty(n, n_x, **f32)
+        FO = torch.empty(n, W, **f32)
+        XC = torch.empty(Lc, n, W, **f32)
+        GC = torch.empty(Lc, n, W, **f32)
+        GH = torch.empty(n, 3, **f32)
+        GV = torch.empty(n, **f32)
+        bufs = (C.c_void_p * 9)(*[t.data_ptr() for t in (E4, XS, GS, XC0, FO, XC, GC, GH, GV)])
+        lib = L.lib()
+        h = net._train_field(device)
+        stream = L.stream_ptr(device)
+        with torch.cuda.device(device):
+            if from_rays:
+                L.check(lib.neddf_neus_train_backward_rays(
+                    h, L.ptr(a), L.ptr(b), L.ptr(c), B, S, L.SAMPLING_IDS[sampling_type], ray_radius, L.ptr(g_sdf),
+                    L.ptr(g_density), L.ptr(g_color), L.ptr(g_normal), bufs, stream), "neus_train_backward_rays")
+            else:
+                L.check(lib.neddf_neus_train_backward(
+                    h, L.ptr(a), L.ptr(b), n, L.ptr(g_sdf), L.ptr(g_density), L.ptr(g_color), L.ptr(g_normal), bufs, stream),
+                    "neus_train_backward")
+            ws = getattr(net, "_wgrad_ws", None)
+            if ws is None or ws.device != device:
+                ws = torch.empty(int(lib.neddf_wgrad_workspace_bytes()) // 4, **f32)
+                net._wgrad_ws = ws
+
+            def wgrad_into(out, row0, A, lda, ka, Bm, rows):
+                """out[row0 : row0 + ka, :256] = A[:, :ka]^T Bm (rows x 256), 128 columns of A at a time."""
+                for c0 in range(0, ka, 128):
+                    kk = min(128, ka - c0)
+                    L.check(lib.neddf_wgrad(L.ptr(A), lda, c0, kk, L.ptr(Bm), W, rows,
+                                            C.c_void_p(out.data_ptr() + 4 * (row0 + c0) * out.shape[1]), out.shape[1], W,
+                                            L.ptr(ws), stream), "wgrad")
+
+            def colsum(Gm, stride):
+                out = torch.empty(W, **f32)
+                L.check(lib.neddf_colsum_value_rows(L.ptr(Gm), n, stride, L.ptr(out), L.ptr(ws), stream), "colsum")
+                return out
+
+            def layer_grad(parts, Gm, rows, stride):
+                """d weight [out, in] and d bias of a layer with inputs `parts` (A, columns) over `rows` rows."""
+                gWt = torch.empty(sum(k for _, k in parts), W, **f32)
+                row0 = 0
+                for Xp, k_in in parts:
+                    wgrad_into(gWt, row0, Xp, k_in, k_in, Gm, rows)
+                    row0 += k_in
+                return [gWt.t().contiguous(), colsum(Gm, stride)]
+
+            grads = []
+            for l in range(Ls):  # layers_sdf.l over the 4 rows of every sample: in_0 = E4, in_l = [XS_{l-1} | E4 if skip]
+                parts = [(E4, n_e)] if l == 0 else ([(XS[l - 1], W)] + ([(E4, n_e)] if (l - 1) in net.skips else []))
+                grads += layer_grad(parts, GS[l], 4 * n, 4 * W)
+            grads += layer_grad([(XC0, n_x), (FO, W)], GC[0], n, W)  # layers_col.0: [pos | dir PE | normal | F]
+            for l in range(1, Lc):
+                grads += layer_grad([(XC[l - 1], W)], GC[l], n, W)
+            gh = torch.empty(3, W, **f32)  # the 3-channel output layer: GH^T h_{Lc-1}, already [out, in]
+            wgrad_into(gh, 0, GH, 3, 3, XC[Lc - 1], n)
+            grads += [gh, GH.sum(0), GV.sum()]
+        return (None,) * 7 + tuple(grads)
 
 
 class NeuS(BaseNeuralField):
@@ -64,6 +169,11 @@ class NeuS(BaseNeuralField):
         self._handle_device = None
         self._packed_key = None
         self._profile_events = None
+        # training backward (csrc/neus_train.cu): opt-in, the default stays the forward-only refusal
+        self.training_kernels = os.environ.get("NEDDF_NEUS_TRAIN", "0") not in ("", "0")
+        self._train_handle = None
+        self._train_handle_device = None
+        self._train_packed_key = None
 
     # ------------------------------------------------------------------ kernel plumbing --
     def _ordered_layers(self) -> List[nn.Linear]:
@@ -82,10 +192,43 @@ class NeuS(BaseNeuralField):
             c.skips[i] = s
         return c
 
+    def _param_tensors(self) -> List[Tensor]:
+        return [p for l in self._ordered_layers() for p in (l.weight, l.bias)] + [self.variance]
+
+    def _train_field(self, device: torch.device):
+        """Handle of the training-backward kernel (forward + transposed weight packs), re-packed when a parameter changed
+        (keyed on the tensors' version counters, like _field)."""
+        lib = L.lib()
+        if self._train_handle is None or self._train_handle_device != device:
+            self._release_train()
+            h = C.c_void_p()
+            with torch.cuda.device(device):
+                cfg = self._config_struct()
+                L.check(lib.neddf_neus_train_create(C.byref(cfg), C.byref(h)), "neus_train_create")
+            self._train_handle, self._train_handle_device = h, device
+        layers = self._ordered_layers()
+        key = tuple((p.data_ptr(), p._version) for p in self._param_tensors())
+        if key != self._train_packed_key:
+            n = len(layers)
+            ws = (C.c_void_p * n)(*[l.weight.data_ptr() for l in layers])
+            bs = (C.c_void_p * n)(*[l.bias.data_ptr() for l in layers])
+            with torch.cuda.device(device):
+                L.check(lib.neddf_neus_train_set_weights(self._train_handle, ws, bs, n, L.ptr(self.variance),
+                                                         L.stream_ptr(device)), "neus_train_set_weights")
+            self._train_packed_key = key
+        return self._train_handle
+
+    def _release_train(self) -> None:
+        if self._train_handle is not None:
+            L.lib().neddf_neus_train_destroy(self._train_handle)
+        self._train_handle, self._train_handle_device, self._train_packed_key = None, None, None
+
     def _release(self) -> None:
         if self._handle is not None:
             L.lib().neddf_neus_destroy(self._handle)
         self._handle, self._handle_device, self._packed_key = None, None, None
+        if getattr(self, "_train_handle", None) is not None:
+            self._release_train()
 
     def __del__(self):
         try:
@@ -124,24 +267,46 @@ class NeuS(BaseNeuralField):
     def _apply(self, fn, *a, **k):
         r = super()._apply(fn, *a, **k)
         self._packed_key = None  # .to()/.cuda() replaced the parameter storage
+        self._train_packed_key = None
         return r
 
     def invalidate(self) -> None:
         self._packed_key = None
+        self._train_packed_key = None
 
     def __getstate__(self):
         d = self.__dict__.copy()
         d["_handle"], d["_handle_device"], d["_packed_key"], d["_profile_events"] = None, None, None, None
+        d["_train_handle"], d["_train_handle_device"], d["_train_packed_key"] = None, None, None
+        d.pop("_wgrad_ws", None)
         return d
 
     def check_engine_status(self) -> None:
         """(fp32 kernel: no range checks to report)"""
 
-    def _refuse_autograd(self) -> None:
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+    def _wants_grad(self) -> bool:
+        """Autograd is recording and some parameter is trainable.  Without the opt-in that is refused."""
+        if not (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())):
+            return False
+        if not self.training_kernels:
             raise NotImplementedError(
-                "neddf_b200.NeuS is forward-only on the CUDA path (no backward kernel for this variant): wrap the call "
-                "in torch.no_grad() / use render_image, or train with the reference and load the checkpoint")
+                "neddf_b200.NeuS is forward-only on the CUDA path by default: wrap the call in torch.no_grad() / use "
+                "render_image, or opt in to the training backward kernel (csrc/neus_train.cu) with "
+                "net.training_kernels = True or NEDDF_NEUS_TRAIN=1")
+        return True
+
+    def _launch_forward(self, a: Tensor, b: Tensor, c, sampling_type, ray_radius: float, with_normal: bool) -> Dict[str, Tensor]:
+        """The inference kernel on rays (sampling_type given) or explicit samples; called under no_grad."""
+        if sampling_type is not None:
+            return self.forward_rays(a, b, c, sampling_type, ray_radius, with_normal=with_normal)
+        return self.forward(Sampling(a, b, a), with_normal=with_normal)
+
+    def _forward_autograd(self, a: Tensor, b: Tensor, c, sampling_type, ray_radius: float, with_normal: bool) -> Dict[str, Tensor]:
+        res = _NeusTrainFn.apply(self, a, b, c, sampling_type, float(ray_radius), with_normal, *self._param_tensors())
+        out = {"sdf": res[0], "density": res[1], "color": res[2]}
+        if with_normal:
+            out["normal"] = res[3]
+        return out
 
     @staticmethod
     def _outputs(B: int, S: int, device, with_normal: bool) -> Dict[str, Tensor]:
@@ -156,10 +321,12 @@ class NeuS(BaseNeuralField):
     def forward(self, sampling: Sampling, with_normal: bool = False) -> Dict[str, Tensor]:
         """neus.py:101-162: {'sdf': [B,S], 'density': [B,S], 'color': [B,S,3]}; ``with_normal`` adds the gradient
         d sdf / d position [B,S,3] that the reference feeds to the colour trunk (neus.py:133-146) but does not return."""
-        self._refuse_autograd()
+        wants_grad = self._wants_grad()
         pos = L.require_cuda_f32(sampling.sample_pos, "sample_pos")
         sdir = L.require_cuda_f32(sampling.sample_dir, "sample_dir")
         B, S = pos.shape[0], pos.shape[1]
+        if wants_grad:
+            return self._forward_autograd(pos.reshape(B, S, 3), sdir.reshape(B, S, 3), None, None, 0.0, with_normal)
         device = pos.device
         out = self._outputs(B, S, device, with_normal)
         h = self._field(device)
@@ -173,10 +340,12 @@ class NeuS(BaseNeuralField):
                      need_penalty: bool = True, need_aux: bool = True, with_normal: bool = False) -> Dict[str, Tensor]:
         """Same network with the sample geometry fused into the kernel (what NeRFRender calls; this variant has
         neither penalties nor auxiliary fields, the flags are accepted for interface parity)."""
-        self._refuse_autograd()
+        wants_grad = self._wants_grad()
         ray_dir = L.require_cuda_f32(ray_dir, "ray_dir")
         ray_orig = L.require_cuda_f32(ray_orig, "ray_orig")
         dists = L.require_cuda_f32(dists, "dists")
+        if wants_grad:
+            return self._forward_autograd(ray_dir, ray_orig, dists, sampling_type, ray_radius, with_normal)
         B, S = dists.shape
         device = dists.device
         out = self._outputs(B, S, device, with_normal)
