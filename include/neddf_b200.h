@@ -473,6 +473,25 @@ int32_t neddf_neus_train_backward_rays(const neddf_neus_train_t* h, const float*
                                        float ray_radius, const float* d_g_sdf, const float* d_g_density, const float* d_g_color,
                                        const float* d_g_normal, float* const* d_bufs, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Marching cubes on a device volume (csrc/mcubes.cu; the reference meshes voxelize's grid with PyMCubes,
+ * scripts/fields_visualizer.py:528-567).  d_volume: fp32 [n0, n1, n2], each dimension in [2, 512].  Index space:
+ * vertex (i, j, k) addresses d_volume[i, j, k]; a corner is inside iff v < threshold; a cube with a non-finite corner
+ * emits nothing.  The case table (csrc/mc_table.cuh, generated by neddf_b200/mc_table.py) is face-consistent, so a
+ * closed level set gives a closed, edge-manifold mesh; triangle normals (v1 - v0) x (v2 - v0) point toward increasing
+ * value.  Vertices are ordered by (grid point, axis) of their edge, faces by (cube, table order): the output is
+ * deterministic.  Two calls with the same volume, threshold and workspace:
+ *   neddf_mc_count  classifies every cube and writes d_totals[0] = V (vertices), d_totals[1] = F (faces);
+ *   neddf_mc_emit   writes d_vertices [V,3] and d_faces [F,3] (int64 vertex ids), reading what count left in the
+ *                   workspace; the caller reads the totals between the two calls to size the outputs.
+ * ------------------------------------------------------------------------------------------------ */
+/* Workspace bytes for a [n0, n1, n2] volume (< 0 on bad sizes). */
+int64_t neddf_mc_workspace_bytes(int32_t n0, int32_t n1, int32_t n2);
+int32_t neddf_mc_count(const float* d_volume, int32_t n0, int32_t n1, int32_t n2, float threshold, void* d_workspace,
+                       int64_t* d_totals, void* stream);
+int32_t neddf_mc_emit(const float* d_volume, int32_t n0, int32_t n1, int32_t n2, float threshold,
+                      const void* d_workspace, float* d_vertices, int64_t* d_faces, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

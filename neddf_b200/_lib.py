@@ -121,6 +121,9 @@ _SIGNATURES = {
     "neddf_neus_train_set_weights": (_I32, [_P, C.POINTER(_P), C.POINTER(_P), _I32, _P, _P]),
     "neddf_neus_train_backward": (_I32, [_P, _P, _P, _I64, _P, _P, _P, _P, C.POINTER(_P), _P]),
     "neddf_neus_train_backward_rays": (_I32, [_P, _P, _P, _P, _I64, _I32, _I32, _F, _P, _P, _P, _P, C.POINTER(_P), _P]),
+    "neddf_mc_workspace_bytes": (_I64, [_I32, _I32, _I32]),
+    "neddf_mc_count": (_I32, [_P, _I32, _I32, _I32, _F, _P, _P, _P]),
+    "neddf_mc_emit": (_I32, [_P, _I32, _I32, _I32, _F, _P, _P, _P, _P]),
 }
 
 _lib = None

@@ -1,0 +1,157 @@
+"""Triangle meshes from a field: marching cubes on the GPU (csrc/mcubes.cu) and a binary PLY writer.
+
+The reference meshes a trained field in its Open3D visualiser (scripts/fields_visualizer.py:528-567): ``voxelize``
+of the distance field, PyMCubes at threshold 0.0275, a ``.dae`` file.  Here the grid, its evaluation and the
+marching cubes stay on the device, and ``python -m neddf_b200.mesh RUN_DIR`` is the headless equivalent:
+
+    python -m neddf_b200.mesh outputs/bunny_smoke [--epoch 2000] [--resolution 64] [--threshold T] [--field NAME]
+                              [--out PATH]
+
+It reads ``RUN_DIR/.hydra/config.yaml``, loads ``RUN_DIR/models/model_{epoch:05}.pth`` into a NeRFRender, meshes
+``get_network()`` with ``extract_mesh`` and writes ``RUN_DIR/mesh/mesh_{resolution}_threshold{threshold}.ply``.
+Defaults per network: NeDDF ``distance`` at 0.0275 (the visualiser's), NeuS ``sdf`` at 0.0; NeRF has no canonical
+level and needs ``--threshold`` (of its ``density`` field).
+"""
+import argparse
+import math
+import os
+import sys
+from typing import Optional, Tuple
+
+import numpy as np
+import torch
+from torch import Tensor
+
+from . import _lib as L
+
+MAX_DIM = 512
+
+
+def marching_cubes(volume: Tensor, threshold: float) -> Tuple[Tensor, Tensor]:
+    """Mesh the level set ``volume == threshold`` of a contiguous fp32 CUDA volume [n0, n1, n2] (each dimension in
+    [2, 512]).  Returns (vertices [V,3] fp32, faces [F,3] int64) on the volume's device.
+
+    Index space, PyMCubes' convention: vertex (i, j, k) addresses ``volume[i, j, k]``.  A corner is inside iff
+    ``v < threshold``; a cube with a non-finite corner emits nothing.  The face-consistent case table makes a closed
+    level set a closed, edge-manifold mesh; the normal ``(v1 - v0) x (v2 - v0)`` points toward increasing value
+    (outward for a distance or SDF, inward for a density).  The output order is deterministic.  Exactly one host
+    synchronisation, to read the vertex and face counts."""
+    if not isinstance(volume, torch.Tensor):
+        raise TypeError("marching_cubes: volume must be a torch.Tensor")
+    if not volume.is_cuda:
+        raise ValueError("marching_cubes: volume must be a CUDA tensor (the kernels have no CPU implementation)")
+    if volume.dtype != torch.float32:
+        raise ValueError(f"marching_cubes: volume must be float32, got {volume.dtype}")
+    if volume.dim() != 3:
+        raise ValueError(f"marching_cubes: volume must be 3-D, got shape {tuple(volume.shape)}")
+    if not volume.is_contiguous():
+        raise ValueError("marching_cubes: volume must be contiguous")
+    n0, n1, n2 = (int(s) for s in volume.shape)
+    if min(n0, n1, n2) < 2 or max(n0, n1, n2) > MAX_DIM:
+        raise ValueError(f"marching_cubes: every dimension must be in [2, {MAX_DIM}], got {(n0, n1, n2)}")
+    thr = float(threshold)
+    if not math.isfinite(thr) or abs(thr) > float(np.finfo(np.float32).max):
+        raise ValueError(f"marching_cubes: threshold must be a finite fp32 value, got {threshold!r}")
+    device = volume.device
+    lib = L.lib()
+    with torch.cuda.device(device):
+        stream = L.stream_ptr(device)
+        n_bytes = L.check(lib.neddf_mc_workspace_bytes(n0, n1, n2), "mc_workspace_bytes")
+        ws = torch.empty(n_bytes, dtype=torch.uint8, device=device)
+        totals = torch.empty(2, dtype=torch.int64, device=device)
+        L.check(lib.neddf_mc_count(L.ptr(volume), n0, n1, n2, thr, L.ptr(ws), L.ptr(totals), stream), "mc_count")
+        n_vert, n_face = (int(v) for v in totals.tolist())
+        vertices = torch.empty(n_vert, 3, dtype=torch.float32, device=device)
+        faces = torch.empty(n_face, 3, dtype=torch.int64, device=device)
+        L.check(lib.neddf_mc_emit(L.ptr(volume), n0, n1, n2, thr, L.ptr(ws), L.ptr(vertices) if n_vert else None,
+                                  L.ptr(faces) if n_face else None, stream), "mc_emit")
+    return vertices, faces
+
+
+def write_ply(path: str, vertices, faces) -> None:
+    """Binary little-endian PLY: float x, y, z per vertex; a ``uchar`` count and int32 indices per face."""
+    v = np.ascontiguousarray(torch.as_tensor(vertices).detach().cpu().numpy(), dtype="<f4").reshape(-1, 3)
+    f = torch.as_tensor(faces).detach().cpu().numpy().reshape(-1, 3)
+    if len(f) and (f.min() < 0 or f.max() >= len(v)):
+        raise ValueError("write_ply: face index out of range")
+    rec = np.empty(len(f), dtype=[("n", "u1"), ("idx", "<i4", (3,))])
+    rec["n"] = 3
+    rec["idx"] = f
+    header = (f"ply\nformat binary_little_endian 1.0\nelement vertex {len(v)}\nproperty float x\nproperty float y\n"
+              f"property float z\nelement face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
+    with open(path, "wb") as fh:
+        fh.write(header.encode("ascii"))
+        fh.write(v.tobytes())
+        fh.write(rec.tobytes())
+
+
+def read_ply(path: str) -> Tuple[np.ndarray, np.ndarray]:
+    """Read back what ``write_ply`` writes: (vertices [V,3] float32, faces [F,3] int64)."""
+    with open(path, "rb") as fh:
+        data = fh.read()
+    end = data.index(b"end_header\n") + len(b"end_header\n")
+    counts = {}
+    for line in data[:end].decode("ascii").splitlines():
+        parts = line.split()
+        if parts[:1] == ["format"] and parts[1] != "binary_little_endian":
+            raise ValueError(f"read_ply: unsupported format {parts[1]}")
+        if parts[:1] == ["element"]:
+            counts[parts[1]] = int(parts[2])
+    nv, nf = counts["vertex"], counts["face"]
+    v = np.frombuffer(data, dtype="<f4", count=3 * nv, offset=end).reshape(nv, 3)
+    rec = np.frombuffer(data, dtype=[("n", "u1"), ("idx", "<i4", (3,))], count=nf, offset=end + 12 * nv)
+    if nf and not (rec["n"] == 3).all():
+        raise ValueError("read_ply: only triangle faces are supported")
+    return v.astype(np.float32), rec["idx"].astype(np.int64)
+
+
+# network class name -> (field, threshold); NeRF has no canonical level
+DEFAULTS = {"NeDDF": ("distance", 0.0275), "NeuS": ("sdf", 0.0), "NeRF": ("density", None)}
+
+
+def mesh_run(run_dir: str, epoch: int = 2000, resolution: int = 64, threshold: Optional[float] = None,
+             field: Optional[str] = None, out: Optional[str] = None, cube_range: float = 1.1,
+             device: str = "cuda:0") -> str:
+    """The headless half of the reference visualiser's main / generate_mesh: returns the written PLY's path."""
+    import yaml
+
+    from .render import NeRFRender
+
+    with open(os.path.join(run_dir, ".hydra", "config.yaml")) as fh:
+        cfg = yaml.safe_load(fh)
+    render_cfg = {k: v for k, v in cfg["render"].items() if k != "_target_"}
+    render = NeRFRender(network_config=cfg["network"], **render_cfg)
+    state = torch.load(os.path.join(run_dir, "models", f"model_{epoch:05}.pth"), map_location="cpu")
+    render.load_state_dict(state)
+    render.to(torch.device(device))
+    net = render.get_network()
+    default_field, default_thr = DEFAULTS[type(net).__name__]
+    field = field or default_field
+    if threshold is None:
+        threshold = default_thr
+    if threshold is None:
+        raise ValueError(f"{type(net).__name__} has no default iso-level: pass --threshold")
+    vertices, faces = net.extract_mesh(field, threshold, cube_range=cube_range, cube_resolution=resolution)
+    if out is None:
+        os.makedirs(os.path.join(run_dir, "mesh"), exist_ok=True)
+        out = os.path.join(run_dir, "mesh", f"mesh_{resolution}_threshold{threshold}.ply")
+    write_ply(out, vertices, faces)
+    return out
+
+
+def main(argv=None) -> None:
+    p = argparse.ArgumentParser(prog="python -m neddf_b200.mesh", description=__doc__.split("\n\n")[0])
+    p.add_argument("run_dir", help="training output directory holding .hydra/config.yaml and models/")
+    p.add_argument("--epoch", type=int, default=2000, help="epoch number of the model file")
+    p.add_argument("--resolution", type=int, default=64, help="grid points per axis (2..512)")
+    p.add_argument("--threshold", type=float, default=None, help="iso-level (default: 0.0275 NeDDF, 0.0 NeuS)")
+    p.add_argument("--field", default=None, help="field to mesh (default: distance NeDDF, sdf NeuS, density NeRF)")
+    p.add_argument("--out", default=None, help="output PLY path (default: RUN_DIR/mesh/mesh_{res}_threshold{thr}.ply)")
+    a = p.parse_args(argv)
+    path = mesh_run(a.run_dir, a.epoch, a.resolution, a.threshold, a.field, a.out)
+    v, f = read_ply(path)
+    print(f"wrote {path}: {len(v)} vertices, {len(f)} faces")
+
+
+if __name__ == "__main__":
+    sys.exit(main())

@@ -11,7 +11,7 @@ update them in place).
 """
 import ctypes as C
 import math
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -199,21 +199,56 @@ class BaseNeuralField(nn.Module):
 
     def voxelize(self, field_name: str = "density", cube_range: float = 1.1, cube_resolution: int = 64,
                  chunk: int = 65536) -> np.ndarray:
-        """Dense-grid evaluation (base_neuralfield.py:49-79); same point order as the reference."""
+        """Dense-grid evaluation (base_neuralfield.py:49-79); same points in the same order as the reference, one
+        device-to-host copy at the end."""
+        return self._grid_volume(field_name, cube_range, cube_resolution, chunk).cpu().numpy()
+
+    def _grid_volume(self, field_name: str, cube_range: float, cube_resolution: int, chunk: int = 65536) -> Tensor:
+        """``voxelize``'s grid evaluated on the device: fp32 [n, n, n] on the module's device.
+
+        The reference builds ``np.meshgrid(ids, ids, ids)`` ('xy' indexing) of ``ids = linspace(-r, r, n)`` and
+        evaluates it in row-major order, so grid point (i, j, k) is at (x, y, z) = (ids[k], ids[i], ids[j]).  Here the
+        positions of each chunk are gathered from the fp32 ``ids`` on the device, with direction (1, 0, 0) and zero
+        variance, through ``self.forward`` in the module's current ``set_iter`` state; no host synchronisation."""
+        n = int(cube_resolution)
+        device = self.device
         with torch.set_grad_enabled(False):
-            ids = np.linspace(-cube_range, cube_range, cube_resolution)
-            zs, ys, xs = np.meshgrid(ids, ids, ids)
-            pos = torch.from_numpy(np.stack([xs.reshape(-1), ys.reshape(-1), zs.reshape(-1)], 1).astype(np.float32))
-            n = cube_resolution ** 3
-            device = self.device
-            result = np.zeros(n, np.float32)
-            one_dir = torch.tensor([[1.0, 0.0, 0.0]])
-            for i in range(0, n, chunk):
-                j = min(n, i + chunk)
-                p = pos[None, i:j, :].to(device)
-                s = Sampling(p, one_dir.expand(j - i, -1)[None].to(device).contiguous(), torch.zeros_like(p))
-                result[i:j] = self.forward(s)[field_name].view(-1).detach().cpu().numpy()
-            return result.reshape(cube_resolution, cube_resolution, cube_resolution)
+            ids = torch.from_numpy(np.linspace(-cube_range, cube_range, n).astype(np.float32)).to(device)
+            total = n ** 3
+            out = torch.empty(total, dtype=torch.float32, device=device)
+            one_dir = torch.tensor([1.0, 0.0, 0.0], device=device)
+            for i in range(0, total, chunk):
+                j = min(total, i + chunk)
+                lin = torch.arange(i, j, device=device)
+                p = torch.stack([ids[lin % n], ids[lin // (n * n)], ids[(lin // n) % n]], 1)[None]
+                s = Sampling(p, one_dir.expand(j - i, 3)[None].contiguous(), torch.zeros_like(p))
+                out[i:j] = self.forward(s)[field_name].reshape(-1)
+            return out.view(n, n, n)
+
+    def extract_mesh(self, field_name: str, threshold: float, cube_range: float = 1.1,
+                     cube_resolution: int = 64) -> Tuple[Tensor, Tensor]:
+        """Triangle mesh of the level set ``field == threshold`` over ``voxelize``'s grid, on the module's device:
+        (vertices [V,3] fp32, faces [F,3] int64).
+
+        The grid is evaluated on the device (``_grid_volume``) and meshed by the marching-cubes kernels
+        (``neddf_b200.mesh.marching_cubes``).  Vertices are returned in the camera frame: grid index (i, j, k) maps to
+        (x, y, z) = (-r + k h, -r + i h, -r + j h) with h = 2r / (n - 1), computed in float64 and rounded to fp32.
+        That map is a cyclic permutation of the axes, so the winding is kept: triangle normals point toward
+        increasing field value, i.e. outward for ``distance`` / ``sdf`` and inward for ``density``.
+
+        The reference's visualiser writes its mesh in a scaled, half-voxel-shifted index space instead
+        (fields_visualizer.py:546-547); that frame is not reproduced here."""
+        from .mesh import marching_cubes
+        n = int(cube_resolution)
+        if n < 2:
+            raise ValueError("extract_mesh: cube_resolution must be >= 2")
+        volume = self._grid_volume(field_name, cube_range, n)
+        vertices, faces = marching_cubes(volume, threshold)
+        h = 2.0 * float(cube_range) / (n - 1)
+        v = vertices.double()
+        r = float(cube_range)
+        world = torch.stack([-r + v[:, 2] * h, -r + v[:, 0] * h, -r + v[:, 1] * h], 1).float()
+        return world, faces
 
 
 class NeDDF(BaseNeuralField):

@@ -1,0 +1,88 @@
+"""Mesh extraction timing: the device grid evaluation (BaseNeuralField._grid_volume, what voxelize and extract_mesh
+run) and the marching-cubes launches (neddf_mc_count, neddf_mc_emit) timed separately with CUDA events after a
+warm-up, with the card's name and power limit read in the same run.
+
+Usage: python tools/mesh_rate.py [resolution=256] [network=bunny|nerf|neus]
+  bunny  the bunny_smoke checkpoint (NeDDF), `distance` at 0.0275
+  nerf   the seeded NeRF golden (case_nerf_relu), `density` at the volume's median
+  neus   the seeded NeuS golden (case_neus_relu), `sdf` at the volume's median
+"""
+import ctypes as C
+import os
+import subprocess
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import torch  # noqa: E402
+
+import neddf_b200  # noqa: E402
+from neddf_b200 import _lib as L  # noqa: E402
+
+res = int(sys.argv[1]) if len(sys.argv) > 1 else 256
+which = sys.argv[2] if len(sys.argv) > 2 else "bunny"
+dev = torch.device("cuda:0")
+if which == "bunny":
+    from tests.helpers import Case
+    c = Case("bunny")
+    render = neddf_b200.NeRFRender(network_config=c.net_cfg, **{k: v for k, v in c.render_cfg.items() if k != "_target_"})
+    render.load_state_dict(c.state_dict())
+    render.to(dev)
+    field, thr = "distance", 0.0275
+elif which == "nerf":
+    from tests.test_nerf_gpu import build
+    from tests.test_nerf_oracle import NerfCase
+    render, field, thr = build(NerfCase("relu"))[0], "density", None
+else:
+    from tests.test_neus_gpu import build
+    from tests.test_neus_oracle import NeusCase
+    render, field, thr = build(NeusCase("relu"))[0], "sdf", None
+net = render.get_network()
+chunk = 1 << 20
+
+
+def timed(fn, reps):
+    fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        out = fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return out, e0.elapsed_time(e1) / reps
+
+
+vol, ms_grid = timed(lambda: net._grid_volume(field, 1.1, res, chunk), 2)
+if thr is None:
+    thr = float(vol.median())
+n0 = n1 = n2 = res
+lib = L.lib()
+stream = L.stream_ptr(dev)
+ws = torch.empty(L.check(lib.neddf_mc_workspace_bytes(n0, n1, n2)), dtype=torch.uint8, device=dev)
+totals = torch.empty(2, dtype=torch.int64, device=dev)
+
+
+def count():
+    L.check(lib.neddf_mc_count(L.ptr(vol), n0, n1, n2, C.c_float(thr), L.ptr(ws), L.ptr(totals), stream), "mc_count")
+
+
+_, ms_count = timed(count, 10)
+n_vert, n_face = totals.tolist()
+verts = torch.empty(max(n_vert, 1), 3, device=dev)
+faces = torch.empty(max(n_face, 1), 3, dtype=torch.int64, device=dev)
+
+
+def emit():
+    L.check(lib.neddf_mc_emit(L.ptr(vol), n0, n1, n2, C.c_float(thr), L.ptr(ws), L.ptr(verts), L.ptr(faces), stream),
+            "mc_emit")
+
+
+_, ms_emit = timed(emit, 10)
+card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                      text=True).stdout.strip()
+print(f"card: {card}")
+print(f"{which} {field} at {thr:g}, {res}^3 grid: {n_vert} vertices, {n_face} faces, workspace {ws.numel() / 2 ** 20:.0f} MiB")
+print(f"grid evaluation ({net.__class__.__name__}, engine {getattr(net, 'engine', '-')}): {ms_grid:.1f} ms, "
+      f"{res ** 3 / ms_grid * 1e3:.3e} points/s")
+print(f"marching cubes: count {ms_count:.2f} ms + emit {ms_emit:.2f} ms = {ms_count + ms_emit:.2f} ms, "
+      f"{(res - 1) ** 3 / (ms_count + ms_emit) * 1e3:.3e} cubes/s")
