@@ -484,6 +484,11 @@ int32_t neddf_neus_train_backward_rays(const neddf_neus_train_t* h, const float*
  *   neddf_mc_count  classifies every cube and writes d_totals[0] = V (vertices), d_totals[1] = F (faces);
  *   neddf_mc_emit   writes d_vertices [V,3] and d_faces [F,3] (int64 vertex ids), reading what count left in the
  *                   workspace; the caller reads the totals between the two calls to size the outputs.
+ *   neddf_mc_normals (optional, after emit, same volume, threshold and workspace) writes d_normals [V,3]: unit
+ *                   area-weighted vertex normals in index space, the sum of the unnormalised face normals
+ *                   (v1 - v0) x (v2 - v0) of the faces using the vertex in ascending face index, every step rounded
+ *                   on its own; a zero-length sum falls back to the vertex's edge axis, signed toward the corner
+ *                   with the larger value.  Deterministic; they point toward increasing value.
  * ------------------------------------------------------------------------------------------------ */
 /* Workspace bytes for a [n0, n1, n2] volume (< 0 on bad sizes). */
 int64_t neddf_mc_workspace_bytes(int32_t n0, int32_t n1, int32_t n2);
@@ -491,6 +496,9 @@ int32_t neddf_mc_count(const float* d_volume, int32_t n0, int32_t n1, int32_t n2
                        int64_t* d_totals, void* stream);
 int32_t neddf_mc_emit(const float* d_volume, int32_t n0, int32_t n1, int32_t n2, float threshold,
                       const void* d_workspace, float* d_vertices, int64_t* d_faces, void* stream);
+int32_t neddf_mc_normals(const float* d_volume, int32_t n0, int32_t n1, int32_t n2, float threshold,
+                         const void* d_workspace, const float* d_vertices, const int64_t* d_faces, float* d_normals,
+                         void* stream);
 
 #ifdef __cplusplus
 }

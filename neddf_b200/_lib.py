@@ -124,6 +124,7 @@ _SIGNATURES = {
     "neddf_mc_workspace_bytes": (_I64, [_I32, _I32, _I32]),
     "neddf_mc_count": (_I32, [_P, _I32, _I32, _I32, _F, _P, _P, _P]),
     "neddf_mc_emit": (_I32, [_P, _I32, _I32, _I32, _F, _P, _P, _P, _P]),
+    "neddf_mc_normals": (_I32, [_P, _I32, _I32, _I32, _F, _P, _P, _P, _P, _P]),
 }
 
 _lib = None

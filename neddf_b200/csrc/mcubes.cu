@@ -4,6 +4,7 @@
 //                 uses), then exclusive scans of the counts (face offsets) and of the flags (vertex ids), then the
 //                 totals V, F into a device int64[2].
 // neddf_mc_emit:  vertices (one thread per edge slot; flagged slots write), faces (one thread per cube).
+// neddf_mc_normals (optional, after emit): area-weighted vertex normals (one thread per edge slot).
 // No host synchronisation between the launches.  Integer scans (CUB DeviceScan) are deterministic, so the output
 // order is fixed: vertices by (grid point, axis), faces by (cube, table order).
 //
@@ -116,6 +117,64 @@ __global__ void __launch_bounds__(kMcThreads) mc_faces(int n0, int n1, int n2, c
   }
 }
 
+// Area-weighted vertex normals, one thread per edge slot; flagged slots write.  Only the (at most 4) cubes that share
+// the slot's edge can use its vertex: they are visited in ascending linear index, each cube's faces in order, so the
+// sum of the unnormalised face normals (v1 - v0) x (v2 - v0) runs in ascending face index.  Every step is rounded on
+// its own (no FMA contraction), so the result is deterministic and a float32 host twin reproduces it bit for bit.
+// A zero-length sum (zero-area faces, or squares that underflow) falls back to the edge axis, signed toward the
+// corner with the larger value: the two corner values differ, exactly one endpoint of a flagged edge is inside.
+__global__ void __launch_bounds__(kMcThreads) mc_normals(const float* __restrict__ vol, int n0, int n1, int n2,
+                                                         const int* __restrict__ offsets, const int* __restrict__ ids,
+                                                         int n_slots, const float* __restrict__ vertices,
+                                                         const int64_t* __restrict__ faces, float* __restrict__ normals) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n_slots) return;
+  const int id = ids[s];
+  if (ids[s + 1] == id) return;
+  const int g = s / 3, axis = s - 3 * g;
+  const int k = g % n2, r = g / n2, j = r % n1, i = r / n1;
+  const int m0 = n0 - 1, m1 = n1 - 1, m2 = n2 - 1;
+  // the cube origin is the edge's grid point minus {0, 1} along each of the two other axes a < b: da on a (the
+  // outer loop), db on b, which visits the cubes in ascending linear index
+  float nx = 0.0f, ny = 0.0f, nz = 0.0f;
+  for (int da = -1; da <= 0; ++da) {
+    for (int db = -1; db <= 0; ++db) {
+      const int ci = i + (axis != 0 ? da : 0);
+      const int cj = j + (axis == 0 ? da : (axis == 2 ? db : 0));
+      const int ck = k + (axis != 2 ? db : 0);
+      if (ci < 0 || ci >= m0 || cj < 0 || cj >= m1 || ck < 0 || ck >= m2) continue;
+      const int c = (ci * m1 + cj) * m2 + ck;
+      const int f1 = offsets[c + 1];
+      for (int f = offsets[c]; f < f1; ++f) {
+        const int64_t* fv = faces + 3 * (int64_t)f;
+        const int64_t i0 = fv[0], i1 = fv[1], i2 = fv[2];
+        if (i0 != id && i1 != id && i2 != id) continue;
+        const float* p0 = vertices + 3 * i0;
+        const float* p1 = vertices + 3 * i1;
+        const float* p2 = vertices + 3 * i2;
+        const float ax = __fsub_rn(p1[0], p0[0]), ay = __fsub_rn(p1[1], p0[1]), az = __fsub_rn(p1[2], p0[2]);
+        const float bx = __fsub_rn(p2[0], p0[0]), by = __fsub_rn(p2[1], p0[1]), bz = __fsub_rn(p2[2], p0[2]);
+        nx = __fadd_rn(nx, __fsub_rn(__fmul_rn(ay, bz), __fmul_rn(az, by)));
+        ny = __fadd_rn(ny, __fsub_rn(__fmul_rn(az, bx), __fmul_rn(ax, bz)));
+        nz = __fadd_rn(nz, __fsub_rn(__fmul_rn(ax, by), __fmul_rn(ay, bx)));
+      }
+    }
+  }
+  const float len = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(nx, nx), __fmul_rn(ny, ny)), __fmul_rn(nz, nz)));
+  float* out = normals + 3 * (int64_t)id;
+  if (len == 0.0f) {
+    const int step = axis == 0 ? n1 * n2 : (axis == 1 ? n2 : 1);
+    const float sign = vol[g + step] > vol[g] ? 1.0f : -1.0f;
+    out[0] = axis == 0 ? sign : 0.0f;
+    out[1] = axis == 1 ? sign : 0.0f;
+    out[2] = axis == 2 ? sign : 0.0f;
+    return;
+  }
+  out[0] = __fdiv_rn(nx, len);
+  out[1] = __fdiv_rn(ny, len);
+  out[2] = __fdiv_rn(nz, len);
+}
+
 int32_t check_dims(int32_t n0, int32_t n1, int32_t n2, const char* who) {
   if (n0 < 2 || n1 < 2 || n2 < 2)
     return fail(NEDDF_E_INVALID, std::string(who) + ": every volume dimension must be >= 2");
@@ -208,6 +267,27 @@ extern "C" int32_t neddf_mc_emit(const float* d_volume, int32_t n0, int32_t n1, 
   mc_vertices<<<blocks(n_slots), kMcThreads, 0, s>>>(d_volume, n1, n2, threshold, ids, n_slots, d_vertices);
   NEDDF_LAUNCH_CHECK();
   mc_faces<<<blocks(l.n_cubes), kMcThreads, 0, s>>>(n0, n1, n2, cases, offsets, ids, d_faces);
+  NEDDF_LAUNCH_CHECK();
+  return NEDDF_OK;
+}
+
+extern "C" int32_t neddf_mc_normals(const float* d_volume, int32_t n0, int32_t n1, int32_t n2, float threshold,
+                                    const void* d_workspace, const float* d_vertices, const int64_t* d_faces,
+                                    float* d_normals, void* stream) {
+  const char* who = "neddf_mc_normals";
+  McLayout l;
+  int32_t rc = layout(n0, n1, n2, l, who);
+  if (rc != NEDDF_OK) return rc;
+  rc = check_call(d_volume, threshold, d_workspace, who);
+  if (rc != NEDDF_OK) return rc;
+  // d_vertices / d_faces / d_normals may be NULL only when V == 0: no thread then reads or writes them
+  cudaStream_t s = (cudaStream_t)stream;
+  const char* ws = (const char*)d_workspace;
+  const int* offsets = (const int*)(ws + l.off_offsets);
+  const int* ids = (const int*)(ws + l.off_ids);
+  const int n_slots = (int)(3 * l.n_points);
+  mc_normals<<<blocks(n_slots), kMcThreads, 0, s>>>(d_volume, n0, n1, n2, offsets, ids, n_slots, d_vertices, d_faces,
+                                                   d_normals);
   NEDDF_LAUNCH_CHECK();
   return NEDDF_OK;
 }

@@ -22,10 +22,15 @@ import numpy as np
 import torch
 
 
+def color_to_uint8(color: torch.Tensor) -> torch.Tensor:
+    """The reference's colour conversion (base_trainer.py:147-160): ``clamp(c * 255, 0, 255)``, then float -> uint8
+    truncates like ``ndarray.astype(np.uint8)`` does for values already clamped to [0, 255]."""
+    return torch.clamp(color * 255, 0, 255).to(torch.uint8)
+
+
 def to_uint8_images(images: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
-    """The reference's conversions (base_trainer.py:147-160) as device ops: float -> uint8 truncates like
-    ``ndarray.astype(np.uint8)`` does for values already clamped to [0, 255]."""
-    rgb = torch.clamp(images["color"] * 255, 0, 255).to(torch.uint8)
+    """The reference's conversions (base_trainer.py:147-160) as device ops."""
+    rgb = color_to_uint8(images["color"])
     depth = torch.clamp((images["depth"] - 2.0) / 4.0 * 50000 / 256, 0, 255).to(torch.uint8)
     return {"rgb": rgb, "depth": depth}
 

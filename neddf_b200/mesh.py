@@ -5,18 +5,19 @@ of the distance field, PyMCubes at threshold 0.0275, a ``.dae`` file.  Here the 
 marching cubes stay on the device, and ``python -m neddf_b200.mesh RUN_DIR`` is the headless equivalent:
 
     python -m neddf_b200.mesh outputs/bunny_smoke [--epoch 2000] [--resolution 64] [--threshold T] [--field NAME]
-                              [--out PATH]
+                              [--out PATH] [--color]
 
 It reads ``RUN_DIR/.hydra/config.yaml``, loads ``RUN_DIR/models/model_{epoch:05}.pth`` into a NeRFRender, meshes
 ``get_network()`` with ``extract_mesh`` and writes ``RUN_DIR/mesh/mesh_{resolution}_threshold{threshold}.ply``.
 Defaults per network: NeDDF ``distance`` at 0.0275 (the visualiser's), NeuS ``sdf`` at 0.0; NeRF has no canonical
-level and needs ``--threshold`` (of its ``density`` field).
+level and needs ``--threshold`` (of its ``density`` field).  ``--color`` adds per-vertex normals and the field's
+colour at every vertex to the PLY (``extract_mesh(..., with_color=True)``).
 """
 import argparse
 import math
 import os
 import sys
-from typing import Optional, Tuple
+from typing import Optional
 
 import numpy as np
 import torch
@@ -27,15 +28,18 @@ from . import _lib as L
 MAX_DIM = 512
 
 
-def marching_cubes(volume: Tensor, threshold: float) -> Tuple[Tensor, Tensor]:
+def marching_cubes(volume: Tensor, threshold: float, normals: bool = False):
     """Mesh the level set ``volume == threshold`` of a contiguous fp32 CUDA volume [n0, n1, n2] (each dimension in
-    [2, 512]).  Returns (vertices [V,3] fp32, faces [F,3] int64) on the volume's device.
+    [2, 512]).  Returns (vertices [V,3] fp32, faces [F,3] int64) on the volume's device; ``normals=True`` adds the
+    unit vertex normals [V,3] fp32 (and leaves vertices and faces bit for bit as they are without it).
 
     Index space, PyMCubes' convention: vertex (i, j, k) addresses ``volume[i, j, k]``.  A corner is inside iff
     ``v < threshold``; a cube with a non-finite corner emits nothing.  The face-consistent case table makes a closed
     level set a closed, edge-manifold mesh; the normal ``(v1 - v0) x (v2 - v0)`` points toward increasing value
-    (outward for a distance or SDF, inward for a density).  The output order is deterministic.  Exactly one host
-    synchronisation, to read the vertex and face counts."""
+    (outward for a distance or SDF, inward for a density).  A vertex normal is the normalised sum of the unnormalised
+    normals of its faces (area weighted), summed in face order with every step rounded on its own; where that sum has
+    zero length it is the vertex's edge axis, signed toward increasing value.  The output order is deterministic.
+    Exactly one host synchronisation, to read the vertex and face counts."""
     if not isinstance(volume, torch.Tensor):
         raise TypeError("marching_cubes: volume must be a torch.Tensor")
     if not volume.is_cuda:
@@ -65,44 +69,98 @@ def marching_cubes(volume: Tensor, threshold: float) -> Tuple[Tensor, Tensor]:
         faces = torch.empty(n_face, 3, dtype=torch.int64, device=device)
         L.check(lib.neddf_mc_emit(L.ptr(volume), n0, n1, n2, thr, L.ptr(ws), L.ptr(vertices) if n_vert else None,
                                   L.ptr(faces) if n_face else None, stream), "mc_emit")
-    return vertices, faces
+        if not normals:
+            return vertices, faces
+        vnormals = torch.empty(n_vert, 3, dtype=torch.float32, device=device)
+        L.check(lib.neddf_mc_normals(L.ptr(volume), n0, n1, n2, thr, L.ptr(ws), L.ptr(vertices) if n_vert else None,
+                                     L.ptr(faces) if n_face else None, L.ptr(vnormals) if n_vert else None, stream),
+                "mc_normals")
+    return vertices, faces, vnormals
 
 
-def write_ply(path: str, vertices, faces) -> None:
-    """Binary little-endian PLY: float x, y, z per vertex; a ``uchar`` count and int32 indices per face."""
+# PLY property types this module writes and reads
+_PLY_TYPES = {"float": "<f4", "uchar": "u1"}
+_XYZ, _NORMAL, _RGB = ("x", "y", "z"), ("nx", "ny", "nz"), ("red", "green", "blue")
+
+
+def _columns(a, dtype, name: str, n: int) -> np.ndarray:
+    c = np.ascontiguousarray(torch.as_tensor(a).detach().cpu().numpy(), dtype=dtype).reshape(-1, 3)
+    if len(c) != n:
+        raise ValueError(f"write_ply: {name} has {len(c)} rows for {n} vertices")
+    return c
+
+
+def write_ply(path: str, vertices, faces, normals=None, colors=None) -> None:
+    """Binary little-endian PLY.  Per vertex, packed: float x, y, z; float nx, ny, nz when ``normals`` is given;
+    uchar red, green, blue when ``colors`` is given.  Float colours are converted by the rule of the project's image
+    writer (``eval_io.color_to_uint8``: clamp(c * 255, 0, 255), truncated); uint8 colours are written as they are.
+    Per face: a ``uchar`` count and int32 indices."""
+    from .eval_io import color_to_uint8
     v = np.ascontiguousarray(torch.as_tensor(vertices).detach().cpu().numpy(), dtype="<f4").reshape(-1, 3)
     f = torch.as_tensor(faces).detach().cpu().numpy().reshape(-1, 3)
     if len(f) and (f.min() < 0 or f.max() >= len(v)):
         raise ValueError("write_ply: face index out of range")
+    props = [(_XYZ, "float", v)]
+    if normals is not None:
+        props.append((_NORMAL, "float", _columns(normals, "<f4", "normals", len(v))))
+    if colors is not None:
+        c = torch.as_tensor(colors).detach()
+        c = c if c.dtype == torch.uint8 else color_to_uint8(c.to(torch.float32))
+        props.append((_RGB, "uchar", _columns(c, "u1", "colors", len(v))))
+    vrec = np.empty(len(v), dtype=[(name, _PLY_TYPES[t]) for names, t, _ in props for name in names])
+    for names, _, cols in props:
+        for q, name in enumerate(names):
+            vrec[name] = cols[:, q]
     rec = np.empty(len(f), dtype=[("n", "u1"), ("idx", "<i4", (3,))])
     rec["n"] = 3
     rec["idx"] = f
-    header = (f"ply\nformat binary_little_endian 1.0\nelement vertex {len(v)}\nproperty float x\nproperty float y\n"
-              f"property float z\nelement face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
+    vprops = "".join(f"property {t} {name}\n" for names, t, _ in props for name in names)
+    header = (f"ply\nformat binary_little_endian 1.0\nelement vertex {len(v)}\n{vprops}"
+              f"element face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
     with open(path, "wb") as fh:
         fh.write(header.encode("ascii"))
-        fh.write(v.tobytes())
+        fh.write(vrec.tobytes())
         fh.write(rec.tobytes())
 
 
-def read_ply(path: str) -> Tuple[np.ndarray, np.ndarray]:
-    """Read back what ``write_ply`` writes: (vertices [V,3] float32, faces [F,3] int64)."""
+def read_ply(path: str, attributes: bool = False):
+    """Read back what ``write_ply`` writes: (vertices [V,3] float32, faces [F,3] int64).  The vertex record is
+    parsed from the header.  ``attributes=True`` returns a dict instead: ``vertices``, ``faces``, and ``normals``
+    [V,3] float32 / ``colors`` [V,3] uint8 when the file has them."""
     with open(path, "rb") as fh:
         data = fh.read()
     end = data.index(b"end_header\n") + len(b"end_header\n")
-    counts = {}
+    counts, vprops, element = {}, [], None
     for line in data[:end].decode("ascii").splitlines():
         parts = line.split()
         if parts[:1] == ["format"] and parts[1] != "binary_little_endian":
             raise ValueError(f"read_ply: unsupported format {parts[1]}")
         if parts[:1] == ["element"]:
-            counts[parts[1]] = int(parts[2])
+            element = parts[1]
+            counts[element] = int(parts[2])
+        if parts[:1] == ["property"] and element == "vertex":
+            if parts[1] not in _PLY_TYPES:
+                raise ValueError(f"read_ply: unsupported vertex property type {parts[1]}")
+            vprops.append((parts[2], _PLY_TYPES[parts[1]]))
     nv, nf = counts["vertex"], counts["face"]
-    v = np.frombuffer(data, dtype="<f4", count=3 * nv, offset=end).reshape(nv, 3)
-    rec = np.frombuffer(data, dtype=[("n", "u1"), ("idx", "<i4", (3,))], count=nf, offset=end + 12 * nv)
+    vrec = np.frombuffer(data, dtype=vprops, count=nv, offset=end)
+    rec = np.frombuffer(data, dtype=[("n", "u1"), ("idx", "<i4", (3,))], count=nf, offset=end + vrec.dtype.itemsize * nv)
     if nf and not (rec["n"] == 3).all():
         raise ValueError("read_ply: only triangle faces are supported")
-    return v.astype(np.float32), rec["idx"].astype(np.int64)
+
+    def cols(names, dtype):
+        return np.stack([vrec[name] for name in names], 1).astype(dtype).reshape(nv, 3)
+
+    v, f = cols(_XYZ, np.float32), rec["idx"].astype(np.int64)
+    if not attributes:
+        return v, f
+    out = {"vertices": v, "faces": f}
+    names = vrec.dtype.names
+    if all(name in names for name in _NORMAL):
+        out["normals"] = cols(_NORMAL, np.float32)
+    if all(name in names for name in _RGB):
+        out["colors"] = cols(_RGB, np.uint8)
+    return out
 
 
 # network class name -> (field, threshold); NeRF has no canonical level
@@ -111,8 +169,9 @@ DEFAULTS = {"NeDDF": ("distance", 0.0275), "NeuS": ("sdf", 0.0), "NeRF": ("densi
 
 def mesh_run(run_dir: str, epoch: int = 2000, resolution: int = 64, threshold: Optional[float] = None,
              field: Optional[str] = None, out: Optional[str] = None, cube_range: float = 1.1,
-             device: str = "cuda:0") -> str:
-    """The headless half of the reference visualiser's main / generate_mesh: returns the written PLY's path."""
+             device: str = "cuda:0", color: bool = False) -> str:
+    """The headless half of the reference visualiser's main / generate_mesh: returns the written PLY's path.
+    ``color=True`` also writes the vertex normals and colours of ``extract_mesh(..., with_color=True)``."""
     import yaml
 
     from .render import NeRFRender
@@ -131,11 +190,11 @@ def mesh_run(run_dir: str, epoch: int = 2000, resolution: int = 64, threshold: O
         threshold = default_thr
     if threshold is None:
         raise ValueError(f"{type(net).__name__} has no default iso-level: pass --threshold")
-    vertices, faces = net.extract_mesh(field, threshold, cube_range=cube_range, cube_resolution=resolution)
+    mesh = net.extract_mesh(field, threshold, cube_range=cube_range, cube_resolution=resolution, with_color=color)
     if out is None:
         os.makedirs(os.path.join(run_dir, "mesh"), exist_ok=True)
         out = os.path.join(run_dir, "mesh", f"mesh_{resolution}_threshold{threshold}.ply")
-    write_ply(out, vertices, faces)
+    write_ply(out, *mesh)
     return out
 
 
@@ -147,8 +206,10 @@ def main(argv=None) -> None:
     p.add_argument("--threshold", type=float, default=None, help="iso-level (default: 0.0275 NeDDF, 0.0 NeuS)")
     p.add_argument("--field", default=None, help="field to mesh (default: distance NeDDF, sdf NeuS, density NeRF)")
     p.add_argument("--out", default=None, help="output PLY path (default: RUN_DIR/mesh/mesh_{res}_threshold{thr}.ply)")
+    p.add_argument("--color", action="store_true",
+                   help="also write vertex normals and the field's colour at every vertex (distance / sdf / density)")
     a = p.parse_args(argv)
-    path = mesh_run(a.run_dir, a.epoch, a.resolution, a.threshold, a.field, a.out)
+    path = mesh_run(a.run_dir, a.epoch, a.resolution, a.threshold, a.field, a.out, color=a.color)
     v, f = read_ply(path)
     print(f"wrote {path}: {len(v)} vertices, {len(f)} faces")
 

@@ -135,6 +135,8 @@ class _NerfTrainFn(torch.autograd.Function):
 
 
 class NeRF(BaseNeuralField):
+    _MESH_VIEW_SIGN = {"density": 1.0}  # density grows inward
+
     def __init__(
         self,
         embed_pos_rank: int = 10,

@@ -11,7 +11,8 @@ update them in place).
 """
 import ctypes as C
 import math
-from typing import Dict, List, Optional, Tuple
+import warnings
+from typing import Dict, List, Optional
 
 import numpy as np
 import torch
@@ -225,8 +226,13 @@ class BaseNeuralField(nn.Module):
                 out[i:j] = self.forward(s)[field_name].reshape(-1)
             return out.view(n, n, n)
 
-    def extract_mesh(self, field_name: str, threshold: float, cube_range: float = 1.1,
-                     cube_resolution: int = 64) -> Tuple[Tensor, Tensor]:
+    # field -> sign of the colour pass's view direction relative to the vertex normal (which points toward increasing
+    # value): -1 for a field that grows outward, +1 for one that grows inward, so the surface is seen from outside.
+    # Only these fields can be meshed with_color.
+    _MESH_VIEW_SIGN: Dict[str, float] = {}
+
+    def extract_mesh(self, field_name: str, threshold: float, cube_range: float = 1.1, cube_resolution: int = 64,
+                     with_color: bool = False):
         """Triangle mesh of the level set ``field == threshold`` over ``voxelize``'s grid, on the module's device:
         (vertices [V,3] fp32, faces [F,3] int64).
 
@@ -236,23 +242,59 @@ class BaseNeuralField(nn.Module):
         That map is a cyclic permutation of the axes, so the winding is kept: triangle normals point toward
         increasing field value, i.e. outward for ``distance`` / ``sdf`` and inward for ``density``.
 
+        ``with_color=True`` returns (vertices, faces, normals [V,3] fp32, colors [V,3] fp32): the kernels' unit
+        area-weighted vertex normals under the same axis permutation (exact: h is isotropic), and the field's
+        ``color`` at every vertex, evaluated through ``forward`` in the module's current ``set_iter`` state with zero
+        variance and a view direction looking at the surface from outside: ``-normal`` for ``distance`` / ``sdf``,
+        ``+normal`` for ``density`` (NeDDF, NeRF).  Any other field raises ValueError.  Vertices and faces are the
+        ``with_color=False`` ones bit for bit.
+
         The reference's visualiser writes its mesh in a scaled, half-voxel-shifted index space instead
         (fields_visualizer.py:546-547); that frame is not reproduced here."""
         from .mesh import marching_cubes
         n = int(cube_resolution)
         if n < 2:
             raise ValueError("extract_mesh: cube_resolution must be >= 2")
+        if with_color and field_name not in self._MESH_VIEW_SIGN:
+            raise ValueError(f"extract_mesh: with_color needs a field that is monotone across the surface; "
+                             f"{type(self).__name__} supports {sorted(self._MESH_VIEW_SIGN)}, got {field_name!r}")
         volume = self._grid_volume(field_name, cube_range, n)
-        vertices, faces = marching_cubes(volume, threshold)
+        if with_color:
+            vertices, faces, index_normals = marching_cubes(volume, threshold, normals=True)
+        else:
+            vertices, faces = marching_cubes(volume, threshold)
         h = 2.0 * float(cube_range) / (n - 1)
         v = vertices.double()
         r = float(cube_range)
         world = torch.stack([-r + v[:, 2] * h, -r + v[:, 0] * h, -r + v[:, 1] * h], 1).float()
-        return world, faces
+        if not with_color:
+            return world, faces
+        normals = index_normals[:, [2, 0, 1]]
+        view_dir = -normals if self._MESH_VIEW_SIGN[field_name] < 0 else normals
+        colors = self._vertex_colors(world, view_dir)
+        if getattr(self, "engine", None) == "auto":
+            try:
+                self.check_engine_status()
+            except EngineRangeError as e:  # engine "auto" left fp16 range: the colours again on the fp32 engine
+                warnings.warn(str(e), RuntimeWarning)
+                colors = self._vertex_colors(world, view_dir)
+        return world, faces, normals, colors
+
+    def _vertex_colors(self, points: Tensor, view_dir: Tensor, chunk: int = 65536) -> Tensor:
+        """``forward(Sampling(points, view_dir, 0))["color"]`` [V,3] in chunks, with no host synchronisation."""
+        with torch.set_grad_enabled(False):
+            out = torch.empty(points.shape[0], 3, dtype=torch.float32, device=points.device)
+            for i in range(0, points.shape[0], chunk):
+                p = points[None, i:i + chunk]
+                s = Sampling(p, view_dir[None, i:i + chunk], torch.zeros_like(p))
+                out[i:i + chunk] = self.forward(s)["color"].reshape(-1, 3)
+            return out
 
 
 class NeDDF(BaseNeuralField):
     """Drop-in for neddf.network.NeDDF (neddf/network/neddf.py:21-326)."""
+
+    _MESH_VIEW_SIGN = {"distance": -1.0, "density": 1.0}  # distance grows outward, density inward
 
     def __init__(
         self,

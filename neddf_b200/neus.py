@@ -127,6 +127,9 @@ class _NeusTrainFn(torch.autograd.Function):
 
 
 class NeuS(BaseNeuralField):
+    # sdf grows outward; density is a bump around the surface, not monotone across it, so it has no outside
+    _MESH_VIEW_SIGN = {"sdf": -1.0}
+
     def __init__(
         self,
         embed_pos_rank: int = 6,

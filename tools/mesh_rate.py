@@ -1,6 +1,7 @@
 """Mesh extraction timing: the device grid evaluation (BaseNeuralField._grid_volume, what voxelize and extract_mesh
-run) and the marching-cubes launches (neddf_mc_count, neddf_mc_emit) timed separately with CUDA events after a
-warm-up, with the card's name and power limit read in the same run.
+run), the marching-cubes launches (neddf_mc_count, neddf_mc_emit), the vertex-normal launch (neddf_mc_normals) and
+the colour pass of extract_mesh(..., with_color=True) timed separately with CUDA events after a warm-up, with the
+card's name and power limit read in the same run.
 
 Usage: python tools/mesh_rate.py [resolution=256] [network=bunny|nerf|neus]
   bunny  the bunny_smoke checkpoint (NeDDF), `distance` at 0.0275
@@ -78,6 +79,24 @@ def emit():
 
 
 _, ms_emit = timed(emit, 10)
+normals = torch.empty(max(n_vert, 1), 3, device=dev)
+
+
+def vertex_normals():
+    L.check(lib.neddf_mc_normals(L.ptr(vol), n0, n1, n2, C.c_float(thr), L.ptr(ws), L.ptr(verts), L.ptr(faces),
+                                 L.ptr(normals), stream), "mc_normals")
+
+
+_, ms_normals = timed(vertex_normals, 10)
+# the colour pass of extract_mesh(..., with_color=True): world positions, view direction against the normal
+sign = net._MESH_VIEW_SIGN.get(field)
+ms_color = None
+if sign is not None and n_vert:
+    h = 2.2 / (res - 1)
+    v64 = verts[:n_vert].double()
+    world = torch.stack([-1.1 + v64[:, 2] * h, -1.1 + v64[:, 0] * h, -1.1 + v64[:, 1] * h], 1).float()
+    view = normals[:n_vert][:, [2, 0, 1]] * sign
+    _, ms_color = timed(lambda: net._vertex_colors(world, view), 10)
 card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                       text=True).stdout.strip()
 print(f"card: {card}")
@@ -86,3 +105,6 @@ print(f"grid evaluation ({net.__class__.__name__}, engine {getattr(net, 'engine'
       f"{res ** 3 / ms_grid * 1e3:.3e} points/s")
 print(f"marching cubes: count {ms_count:.2f} ms + emit {ms_emit:.2f} ms = {ms_count + ms_emit:.2f} ms, "
       f"{(res - 1) ** 3 / (ms_count + ms_emit) * 1e3:.3e} cubes/s")
+print(f"vertex normals: {ms_normals:.3f} ms")
+print(f"colour pass: {ms_color:.3f} ms ({n_vert} vertices)" if ms_color is not None else
+      f"colour pass: {field} has no outside, not run")
