@@ -11,7 +11,6 @@ nerf.py:107-165 with respect to the parameters runs in ``csrc/nerf_train.cu`` (f
 gradients in fp32 FMA) + ``neddf_wgrad`` / ``neddf_colsum_value_rows`` (weight / bias gradients).  That kernel has so far
 been validated through the host emulation of its tile program only (tests/test_nerf_train_emul.py: the real reference's
 autograd gradients, sanitizers) - it was written after the round's GPU budget was spent - hence the opt-in."""
-import ctypes as C
 import math
 import os
 from typing import Dict, List, Optional
@@ -20,6 +19,7 @@ import torch
 from torch import Tensor, nn
 
 from . import _lib as L
+from ._host import KernelHandle, WeightGrad
 from .network import BaseNeuralField
 from .ray import Sampling
 
@@ -91,51 +91,34 @@ class _NerfTrainFn(torch.autograd.Function):
                 L.check(lib.neddf_nerf_train_backward(
                     h, L.fbuf(lowpass), L.ptr(a), L.ptr(b), L.ptr(c), n, L.ptr(g_density), L.ptr(g_color), L.ptr(X), L.ptr(G),
                     L.ptr(E), L.ptr(D), L.ptr(C1), L.ptr(GC1), L.ptr(GZD), stream), "nerf_train_backward")
-            ws = getattr(net, "_wgrad_ws", None)
-            if ws is None or ws.device != device:
-                ws = torch.empty(int(lib.neddf_wgrad_workspace_bytes()) // 4, device=device, dtype=torch.float32)
-                net._wgrad_ws = ws
-
-            def wgrad_into(out, row0, A, lda, ka, Bm, n_cols):
-                """out[row0 : row0 + ka, :n_cols] = A[:, :ka]^T Bm[:, :n_cols] (Bm has 256 columns), 128 columns of A at a time."""
-                for c0 in range(0, ka, 128):
-                    kk = min(128, ka - c0)
-                    L.check(lib.neddf_wgrad(L.ptr(A), lda, c0, kk, L.ptr(Bm), W, n,
-                                            C.c_void_p(out.data_ptr() + 4 * (row0 + c0) * out.shape[1]), out.shape[1], n_cols,
-                                            L.ptr(ws), stream), "wgrad")
-
-            def colsum(Gm):
-                out = torch.empty(W, device=device, dtype=torch.float32)
-                L.check(lib.neddf_colsum_value_rows(L.ptr(Gm), n, W, L.ptr(out), L.ptr(ws), stream), "colsum")
-                return out
-
+            wg = WeightGrad(net, device, n)
             grads = []
             for l in range(Lh):  # layers.l: d W^T [in, 256] = in_l^T G_l with in_0 = E, in_l = [h_{l-1} | E if l-1 in skips]
                 parts = [(E, n_e)] if l == 0 else ([(X[l - 1], W)] + ([(E, n_e)] if (l - 1) in net.skips else []))
-                gWt = torch.empty(sum(k for _, k in parts), W, device=device, dtype=torch.float32)
-                row0 = 0
-                for Xp, k_in in parts:
-                    wgrad_into(gWt, row0, Xp, k_in, k_in, G[l], W)
-                    row0 += k_in
-                grads += [gWt.t().contiguous(), colsum(G[l])]
-            gwd = torch.empty(1, W, device=device, dtype=torch.float32)  # outL_density: GZD^T h_{L-1}
-            wgrad_into(gwd, 0, GZD, 1, 1, X[Lh - 1], W)
+                gWt, gb = wg.layer(parts, G[l], n, W)
+                grads += [gWt.t().contiguous(), gb]
+            gwd = wg.empty(1, W)  # outL_density: GZD^T h_{L-1}
+            wg.into(gwd, 0, GZD, 1, 1, X[Lh - 1], n)
             grads += [gwd, GZD.sum().reshape(1)]
             # (all GEMMs with n_cols = ld_out = 256, the parameters test_wgrad_gemm holds on hardware; the colour branch is
             #  128 wide, the upper half of GC1 / C1 is zero and sliced away)
-            gc1t = torch.empty(W + n_d, W, device=device, dtype=torch.float32)  # outL_color.0: [h_{L-1} | D]^T GC1
-            wgrad_into(gc1t, 0, X[Lh - 1], W, W, GC1, W)
-            wgrad_into(gc1t, W, D, n_d, n_d, GC1, W)
-            grads += [gc1t[:, :W // 2].t().contiguous(), colsum(GC1)[:W // 2].contiguous()]
-            gc2 = torch.empty(3, W, device=device, dtype=torch.float32)  # outL_color.2: g_color^T C1
+            gc1t, gb1 = wg.layer([(X[Lh - 1], W), (D, n_d)], GC1, n, W)  # outL_color.0: [h_{L-1} | D]^T GC1
+            grads += [gc1t[:, :W // 2].t().contiguous(), gb1[:W // 2].contiguous()]
+            gc2 = wg.empty(3, W)  # outL_color.2: g_color^T C1
             g_col2 = g_color.reshape(n, 3)
-            wgrad_into(gc2, 0, g_col2, 3, 3, C1, W)
+            wg.into(gc2, 0, g_col2, 3, 3, C1, n)
             grads += [gc2[:, :W // 2].contiguous(), g_col2.sum(0)]
         return (None, None, None, None, None, None) + tuple(grads)
 
 
 class NeRF(BaseNeuralField):
     _MESH_VIEW_SIGN = {"density": 1.0}  # density grows inward
+    _HANDLES = (KernelHandle("neddf_nerf"), KernelHandle("neddf_nerf_train", "_train"))
+    _GRAD_REFUSAL = (
+        "neddf_b200.NeRF is forward-only on the CUDA path by default: wrap the call in torch.no_grad() / use "
+        "render_image, or train with the reference and load the checkpoint.  The training backward kernel "
+        "(csrc/nerf_train.cu) is opt-in - net.training_kernels = True or NEDDF_NERF_TRAIN=1 - until it has been "
+        "run on hardware (so far: host emulation against the reference's autograd gradients)")
 
     def __init__(
         self,
@@ -170,15 +153,8 @@ class NeRF(BaseNeuralField):
         self.lowpass_alpha = float(lowpass_alpha_offset)
         # kernel-side state
         self.engine = "fp32"  # the only engine of this variant; NeRFRender.set_engine may overwrite the attribute
-        self._handle = None
-        self._handle_device = None
-        self._packed_key = None
-        self._profile_events = None
         # training backward (csrc/nerf_train.cu): opt-in until it has been run on hardware (module docstring)
         self.training_kernels = os.environ.get("NEDDF_NERF_TRAIN", "0") not in ("", "0")
-        self._train_handle = None
-        self._train_handle_device = None
-        self._train_packed_key = None
 
     # ------------------------------------------------------------------ kernel plumbing --
     def _ordered_layers(self) -> List[nn.Linear]:
@@ -187,115 +163,13 @@ class NeRF(BaseNeuralField):
     def _lowpass_list(self) -> List[float]:
         return lowpass_scale(self.embed_pos_rank, self.lowpass_alpha)
 
-    def _train_field(self, device: torch.device):
-        """Handle of the training-backward kernel (forward + transposed weight packs), re-packed when a parameter changed."""
-        lib = L.lib()
-        if self._train_handle is None or self._train_handle_device != device:
-            self._release_train()
-            h = C.c_void_p()
-            with torch.cuda.device(device):
-                cfg = self._config_struct()
-                L.check(lib.neddf_nerf_train_create(C.byref(cfg), C.byref(h)), "nerf_train_create")
-            self._train_handle, self._train_handle_device = h, device
-        layers = self._ordered_layers()
-        key = tuple((p.data_ptr(), p._version) for l in layers for p in (l.weight, l.bias))
-        if key != self._train_packed_key:
-            n = len(layers)
-            ws = (C.c_void_p * n)(*[l.weight.data_ptr() for l in layers])
-            bs = (C.c_void_p * n)(*[l.bias.data_ptr() for l in layers])
-            with torch.cuda.device(device):
-                L.check(lib.neddf_nerf_train_set_weights(self._train_handle, ws, bs, n, L.stream_ptr(device)), "nerf_train_set_weights")
-            self._train_packed_key = key
-        return self._train_handle
-
-    def _release_train(self) -> None:
-        if self._train_handle is not None:
-            L.lib().neddf_nerf_train_destroy(self._train_handle)
-        self._train_handle, self._train_handle_device, self._train_packed_key = None, None, None
-
     def _config_struct(self) -> L.NerfConfig:
         c = L.NerfConfig()
         c.embed_pos_rank, c.embed_dir_rank = self.embed_pos_rank, self.embed_dir_rank
         c.layer_count, c.layer_width = self.layer_count, self.layer_width
         c.activation_type = L.ACT_IDS[self.activation_type]
         c.density_activation_type = L.ACT_IDS[self.density_activation_type]
-        if len(self.skips) > L.MAX_SKIPS:
-            raise NotImplementedError("neddf_b200: more than 8 skip connections")
-        c.n_skips = len(self.skips)
-        for i, s in enumerate(self.skips):
-            c.skips[i] = s
-        return c
-
-    def _release(self) -> None:
-        if self._handle is not None:
-            L.lib().neddf_nerf_destroy(self._handle)
-        self._handle, self._handle_device, self._packed_key = None, None, None
-        if getattr(self, "_train_handle", None) is not None:
-            self._release_train()
-
-    def __del__(self):
-        try:
-            self._release()
-        except Exception:  # interpreter shutdown
-            pass
-
-    def _field(self, device: torch.device):
-        lib = L.lib()
-        if device.type != "cuda":
-            raise RuntimeError("neddf_b200.NeRF runs on CUDA devices only: move the module with .to('cuda') "
-                               "(the hot path has no CPU implementation)")
-        if self._handle is None or self._handle_device != device:
-            self._release()
-            h = C.c_void_p()
-            with torch.cuda.device(device):
-                cfg = self._config_struct()
-                L.check(lib.neddf_nerf_create(C.byref(cfg), C.byref(h)), "nerf_create")
-            self._handle, self._handle_device = h, device
-        layers = self._ordered_layers()
-        key = tuple((p.data_ptr(), p._version) for l in layers for p in (l.weight, l.bias))
-        if key != self._packed_key:
-            for l in layers:
-                if l.weight.dtype != torch.float32 or not l.weight.is_contiguous() or l.weight.device != device:
-                    raise RuntimeError("neddf_b200: parameters must be contiguous fp32 tensors on the module's device")
-            n = len(layers)
-            ws = (C.c_void_p * n)(*[l.weight.data_ptr() for l in layers])
-            bs = (C.c_void_p * n)(*[l.bias.data_ptr() for l in layers])
-            with torch.cuda.device(device):
-                L.check(lib.neddf_nerf_set_weights(self._handle, ws, bs, n, L.stream_ptr(device)), "nerf_set_weights")
-            self._packed_key = key
-        return self._handle
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        self._packed_key = None  # .to()/.cuda() replaced the parameter storage
-        self._train_packed_key = None
-        return r
-
-    def invalidate(self) -> None:
-        self._packed_key = None
-        self._train_packed_key = None
-
-    def __getstate__(self):
-        d = self.__dict__.copy()
-        d["_handle"], d["_handle_device"], d["_packed_key"], d["_profile_events"] = None, None, None, None
-        d["_train_handle"], d["_train_handle_device"], d["_train_packed_key"] = None, None, None
-        d.pop("_wgrad_ws", None)
-        return d
-
-    def check_engine_status(self) -> None:
-        """(fp32 kernel: no range checks to report)"""
-
-    def _wants_grad(self) -> bool:
-        """Autograd is recording and some parameter is trainable.  Without the opt-in that is refused."""
-        if not (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())):
-            return False
-        if not self.training_kernels:
-            raise NotImplementedError(
-                "neddf_b200.NeRF is forward-only on the CUDA path by default: wrap the call in torch.no_grad() / use "
-                "render_image, or train with the reference and load the checkpoint.  The training backward kernel "
-                "(csrc/nerf_train.cu) is opt-in - net.training_kernels = True or NEDDF_NERF_TRAIN=1 - until it has been "
-                "run on hardware (so far: host emulation against the reference's autograd gradients)")
-        return True
+        return self._fill_skips(c)
 
     def _launch_forward(self, a: Tensor, b: Tensor, c: Tensor, sampling_type, ray_radius: float) -> Dict[str, Tensor]:
         """The inference kernels on rays (sampling_type given) or explicit samples; called under no_grad."""
@@ -304,8 +178,7 @@ class NeRF(BaseNeuralField):
         return self.forward(Sampling(a, b, c))
 
     def _forward_autograd(self, a: Tensor, b: Tensor, c: Tensor, sampling_type, ray_radius: float) -> Dict[str, Tensor]:
-        flat = [t for l in self._ordered_layers() for t in (l.weight, l.bias)]
-        density, color = _NerfTrainFn.apply(self, a, b, c, sampling_type, float(ray_radius), *flat)
+        density, color = _NerfTrainFn.apply(self, a, b, c, sampling_type, float(ray_radius), *self._param_tensors())
         return {"density": density, "color": color}
 
     def _lowpass(self):
@@ -344,17 +217,10 @@ class NeRF(BaseNeuralField):
         out = {"density": torch.empty(B, S, device=device, dtype=torch.float32),
                "color": torch.empty(B, S, 3, device=device, dtype=torch.float32)}
         h = self._field(device)
-        prof = self._profile_events
-        if prof is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record(torch.cuda.current_stream(device))
-        with torch.cuda.device(device):
+        with self._profiled(device, B * S), torch.cuda.device(device):
             L.check(L.lib().neddf_nerf_forward_rays(h, self._lowpass(), L.ptr(ray_dir), L.ptr(ray_orig), L.ptr(dists), B, S,
                                                     L.SAMPLING_IDS[sampling_type], float(ray_radius), L.ptr(out["density"]),
                                                     L.ptr(out["color"]), L.stream_ptr(device)), "nerf_forward_rays")
-        if prof is not None:
-            e1.record(torch.cuda.current_stream(device))
-            prof.append((e0, e1, B * S))
         return out
 
     def set_iter(self, iter: int) -> None:

@@ -9,16 +9,17 @@ arithmetic of ``forward`` happens in libneddf_b200.so (neddf_field_forward*); th
 are re-packed into kernel layout whenever their version counters change (optimiser steps
 update them in place).
 """
+import contextlib
 import ctypes as C
-import math
 import warnings
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 import torch
 from torch import Tensor, nn
 
 from . import _lib as L
+from ._host import KernelHandle, WeightGrad
 from .ray import Sampling
 
 
@@ -134,27 +135,13 @@ class _FieldTrainFn(torch.autograd.Function):
                     L.ptr(xes), L.ptr(xcol), L.stream_ptr(device)), "field_backward_samples")
 
         # weight gradients gW = X^T G over the 4N rows (linear.py:76-79) and bias gradients (sum over the value
-        # rows): tensor-core split-K GEMMs of this library (csrc/wgrad.cu), written straight into the gradient
-        # tensors - no library GEMM on the training path
-        lib = L.lib()
-        stream = L.stream_ptr(device)
-        ws = getattr(net, "_wgrad_ws", None)
-        if ws is None or ws.device != device:
-            ws = torch.empty(int(lib.neddf_wgrad_workspace_bytes()) // 4, device=device, dtype=torch.float32)
-            net._wgrad_ws = ws
+        # rows): tensor-core split-K GEMMs of this library (WeightGrad), written straight into the gradient tensors - no
+        # vendor GEMM on the training path
+        wg = WeightGrad(net, device, n)
         R = 4 * n
-
-        def wgrad_into(out, row0, A, lda, ka, Bm, n_cols=256):
-            """out[row0 : row0 + ka, :n_cols] = A[:, :ka]^T Bm, in 128-column tiles of A."""
-            for c0 in range(0, ka, 128):
-                kk = min(128, ka - c0)
-                L.check(lib.neddf_wgrad(L.ptr(A), lda, c0, kk, L.ptr(Bm), 256, R,
-                                        C.c_void_p(out.data_ptr() + 4 * (row0 + c0) * out.shape[1]), out.shape[1], n_cols,
-                                        L.ptr(ws), stream), "wgrad")
-
         grads = []
         with torch.cuda.device(device):
-            for l in range(n_hidden):
+            for l in range(n_hidden):  # the weights are [in, out]: X^T G is the gradient as it stands
                 if l == 0:
                     parts = [(xes, n_e0)]
                 elif l < n_ddf:
@@ -163,19 +150,12 @@ class _FieldTrainFn(torch.autograd.Function):
                     parts = [(xcol, off_h), (post[n_ddf - 1], 256)]
                 else:
                     parts = [(post[l - 1], 256)]
-                gW = torch.empty(sum(k for _, k in parts), 256, device=device, dtype=torch.float32)
-                row0 = 0
-                for X, k_in in parts:
-                    wgrad_into(gW, row0, X, k_in, k_in, gpre[l])
-                    row0 += k_in
-                gb = torch.empty(256, device=device, dtype=torch.float32)
-                L.check(lib.neddf_colsum_value_rows(L.ptr(gpre[l]), n, 4 * 256, L.ptr(gb), L.ptr(ws), stream), "colsum")
-                grads += [gW, gb]
+                grads += wg.layer(parts, gpre[l], R, 4 * 256)
             # heads: gW^T [outs, 256] = ghead^T post (the 2- / 3-column head gradients are the A operand)
-            gda_t = torch.empty(2, 256, device=device, dtype=torch.float32)
-            wgrad_into(gda_t, 0, ghead_da, 2, 2, post[n_ddf - 1])
-            gc_t = torch.empty(3, 256, device=device, dtype=torch.float32)
-            wgrad_into(gc_t, 0, ghead_col, 4, 3, post[n_hidden - 1])
+            gda_t = wg.empty(2, 256)
+            wg.into(gda_t, 0, ghead_da, 2, 2, post[n_ddf - 1], R)
+            gc_t = wg.empty(3, 256)
+            wg.into(gc_t, 0, ghead_col, 4, 3, post[n_hidden - 1], R)
         b_da = ghead_da[:, 0, :].sum(0)
         grads += [gda_t[0].reshape(256, 1).contiguous(), b_da[0:1].contiguous(), gda_t[1].reshape(256, 1).contiguous(),
                   b_da[1:2].contiguous()]
@@ -189,7 +169,95 @@ class EngineRangeError(FloatingPointError):
 
 
 class BaseNeuralField(nn.Module):
-    """neddf/network/base_neuralfield.py:11-79."""
+    """neddf/network/base_neuralfield.py:11-79, plus the kernel plumbing the CUDA networks share: their C handles (one
+    ``KernelHandle`` per kind in ``_HANDLES``: the forward handle, then the training one if any), the opt-in refusal of
+    autograd and the CUDA-event bracket bench.py reads."""
+
+    _HANDLES: Tuple[KernelHandle, ...] = ()
+    _GRAD_REFUSAL: Optional[str] = None  # set for a network whose training backward is opt-in (``training_kernels``)
+
+    def __init__(self) -> None:
+        super().__init__()
+        for h in self._HANDLES:
+            h.reset(self)
+        self._profile_events = None  # bench.py: list receiving (start, end, n_evaluations or None) CUDA events
+
+    def _field(self, device: torch.device):
+        """Forward handle with weights packed for the parameters' current values."""
+        if device.type != "cuda":
+            raise RuntimeError(f"neddf_b200.{type(self).__name__} runs on CUDA devices only: move the module with "
+                               ".to('cuda') (the hot path has no CPU implementation)")
+        return self._HANDLES[0].get(self, device)
+
+    def _train_field(self, device: torch.device):
+        """Handle of the training-backward kernel (NeRF, NeuS), re-packed like ``_field``'s."""
+        return self._HANDLES[1].get(self, device)
+
+    def _param_tensors(self) -> List[Tensor]:
+        """The tensors the kernel packs are keyed on: weight and bias of every layer of ``_ordered_layers``."""
+        return [t for l in self._ordered_layers() for t in (l.weight, l.bias)]
+
+    def _fill_skips(self, cfg):
+        if len(self.skips) > L.MAX_SKIPS:
+            raise NotImplementedError("neddf_b200: more than 8 skip connections")
+        cfg.n_skips = len(self.skips)
+        for i, s in enumerate(self.skips):
+            cfg.skips[i] = s
+        return cfg
+
+    def _release(self) -> None:
+        for h in self._HANDLES:
+            h.release(self)
+
+    def __del__(self):
+        try:
+            self._release()
+        except Exception:  # interpreter shutdown: torch internals may already be gone
+            pass
+
+    def _apply(self, fn, *a, **k):
+        r = super()._apply(fn, *a, **k)
+        self.invalidate()  # .to()/.cuda() replaced the parameter storage
+        return r
+
+    def invalidate(self) -> None:
+        """Force a re-pack of the kernel-layout weights on the next call.  Needed only after edits that
+        bypass the parameters' version counters (``p.data.copy_(...)``, EMA swaps through ``.data``);
+        optimiser steps, ``load_state_dict`` and ``.to()`` are detected automatically."""
+        for h in self._HANDLES:
+            setattr(self, h.names[2], None)
+
+    # the kernel handles are process-local pointers: copies and pickles get fresh ones lazily
+    def __getstate__(self):
+        d = self.__dict__.copy()
+        d.update({name: None for h in self._HANDLES for name in h.names})
+        d["_profile_events"] = None
+        d.pop("_wgrad_ws", None)
+        return d
+
+    def check_engine_status(self) -> None:
+        """(fp32 kernel: no range checks to report)"""
+
+    def _wants_grad(self) -> bool:
+        """Autograd is recording and some parameter is trainable.  Without the opt-in that is refused."""
+        if not (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())):
+            return False
+        if self._GRAD_REFUSAL is not None and not self.training_kernels:
+            raise NotImplementedError(self._GRAD_REFUSAL)
+        return True
+
+    @contextlib.contextmanager
+    def _profiled(self, device: torch.device, n_evaluations: Optional[int]):
+        """Brackets a launch with CUDA events appended to ``_profile_events`` when it is a list."""
+        prof = self._profile_events
+        if prof is None:
+            yield
+            return
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(torch.cuda.current_stream(device))
+        yield
+        e1.record(torch.cuda.current_stream(device))
+        prof.append((e0, e1, n_evaluations))
 
     @property
     def device(self) -> torch.device:
@@ -295,6 +363,7 @@ class NeDDF(BaseNeuralField):
     """Drop-in for neddf.network.NeDDF (neddf/network/neddf.py:21-326)."""
 
     _MESH_VIEW_SIGN = {"distance": -1.0, "density": 1.0}  # distance grows outward, density inward
+    _HANDLES = (KernelHandle("neddf_field"),)
 
     def __init__(
         self,
@@ -352,10 +421,6 @@ class NeDDF(BaseNeuralField):
         # kernel-side state
         self.engine = "auto"          # "auto" | "fp32" | "tc" | "tc2"
         self._range_fallback = False  # "auto" met an activation outside fp16 range: it resolves to fp32 from then on
-        self._handle = None
-        self._handle_device = None
-        self._packed_key = None
-        self._profile_events = None   # bench.py: list receiving (start, end, n_evaluations) CUDA events
 
     def resolved_engine(self, device=None) -> str:
         """Engine that will actually run for ``self.engine`` ("fp32" or "tc")."""
@@ -380,11 +445,7 @@ class NeDDF(BaseNeuralField):
         c.activation_type = L.ACT_IDS[self.activation_type]
         c.density_activation_type = L.ACT_IDS[self.density_activation_type]
         c.d_near = self.d_near
-        if len(self.skips) > L.MAX_SKIPS:
-            raise NotImplementedError("neddf_b200: more than 8 skip connections")
-        c.n_skips = len(self.skips)
-        for i, s in enumerate(self.skips):
-            c.skips[i] = s
+        self._fill_skips(c)
         for i, k in enumerate(L.PENALTY_KEYS):  # absent key -> unweighted, neddf.py:296-299
             c.penalty_weight[i] = self.penalty_weight.get(k, 1.0)
         return c
@@ -395,77 +456,6 @@ class NeDDF(BaseNeuralField):
         pw = (C.c_float * L.N_PENALTY)(*[float(self.penalty_weight.get(k, 1.0)) for k in L.PENALTY_KEYS])
         return L.FieldState(float(self.aux_grad_scale), float(self.distance_range_max), float(self.lowpass_alpha), pw)
 
-    def _release(self) -> None:
-        if self._handle is not None:
-            try:
-                L.lib().neddf_field_destroy(self._handle)
-            except Exception:  # interpreter shutdown
-                pass
-            self._handle = None
-            self._packed_key = None
-
-    def __del__(self):
-        try:
-            self._release()
-        except Exception:  # interpreter shutdown: torch internals may already be gone
-            pass
-
-    def _field(self, device: torch.device):
-        """Handle with weights packed for the parameters' current values."""
-        lib = L.lib()
-        if device.type != "cuda":
-            raise RuntimeError("neddf_b200.NeDDF runs on CUDA devices only: move the module with .to('cuda') "
-                               "(the hot path has no CPU implementation)")
-        if self._handle is None or self._handle_device != device:
-            self._release()
-            h = C.c_void_p()
-            with torch.cuda.device(device):
-                cfg = self._config_struct()
-                L.check(lib.neddf_field_create(C.byref(cfg), C.byref(h)), "field_create")
-            self._handle, self._handle_device = h, device
-        layers = self._ordered_layers()
-        key = tuple((p.data_ptr(), p._version) for l in layers for p in (l.weight, l.bias))
-        if key != self._packed_key:
-            n = len(layers)
-            ws = (C.c_void_p * n)(*[l.weight.data_ptr() for l in layers])
-            bs = (C.c_void_p * n)(*[l.bias.data_ptr() for l in layers])
-            for l in layers:
-                if l.weight.dtype != torch.float32 or not l.weight.is_contiguous() or l.weight.device != device:
-                    raise RuntimeError("neddf_b200: parameters must be contiguous fp32 tensors on the module's device")
-            with torch.cuda.device(device):
-                L.check(lib.neddf_field_set_weights(self._handle, ws, bs, n, L.stream_ptr(device)), "field_set_weights")
-            self._packed_key = key
-        return self._handle
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        self._packed_key = None  # .to()/.cuda() replaced the parameter storage
-        return r
-
-    def invalidate(self) -> None:
-        """Force a re-pack of the kernel-layout weights on the next call.  Needed only after edits that
-        bypass the parameters' version counters (``p.data.copy_(...)``, EMA swaps through ``.data``);
-        optimiser steps, ``load_state_dict`` and ``.to()`` are detected automatically."""
-        self._packed_key = None
-
-    # the kernel handle is a process-local pointer: copies and pickles get a fresh one lazily
-    def __getstate__(self):
-        d = self.__dict__.copy()
-        d["_handle"] = None
-        d["_handle_device"] = None
-        d["_packed_key"] = None
-        d["_profile_events"] = None
-        return d
-
-    def __deepcopy__(self, memo):
-        import copy
-        cls = self.__class__
-        new = cls.__new__(cls)
-        memo[id(self)] = new
-        for k, v in self.__getstate__().items():
-            new.__dict__[k] = copy.deepcopy(v, memo)
-        return new
-
     # ------------------------------------------------------------------------- forward --
     def forward(self, sampling: Sampling) -> Dict[str, Tensor]:
         """NeDDF.forward (neddf.py:162-309): Sampling[B,S,3] -> distance, density, color,
@@ -473,15 +463,13 @@ class NeDDF(BaseNeuralField):
         parameters through density / color / fields_penalty; distance and aux_grad are returned
         without a graph - no loss of the reference consumes them)."""
         pos = sampling.sample_pos
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            B, S = pos.shape[0], pos.shape[1]
+        B, S = pos.shape[0], pos.shape[1]
+        if self._wants_grad():
             p3 = L.require_cuda_f32(pos.reshape(B, S, 3), "sample_pos")
             d3 = L.require_cuda_f32(sampling.sample_dir.reshape(B, S, 3), "sample_dir")
             v3 = L.require_cuda_f32(sampling.diag_variance.reshape(B, S, 3), "diag_variance")
-            flat = [t for l in self._ordered_layers() for t in (l.weight, l.bias)]
-            d, c, pnl, dist, aux = _FieldTrainFn.apply(self, p3, d3, v3, None, 0.0, *flat)
+            d, c, pnl, dist, aux = _FieldTrainFn.apply(self, p3, d3, v3, None, 0.0, *self._param_tensors())
             return {"distance": dist, "density": d, "color": c, "fields_penalty": pnl, "aux_grad": aux}
-        B, S = pos.shape[0], pos.shape[1]
         device = pos.device
         # reshape, not view: accept the expanded tensors the reference's point sampler returns
         p3 = L.require_cuda_f32(pos.reshape(-1, 3), "sample_pos")
@@ -509,16 +497,13 @@ class NeDDF(BaseNeuralField):
         """Same network with the sample geometry fused into the kernel prologue (no [N,3]
         Sampling tensors in HBM).  Used by NeRFRender.  Under autograd (training) it runs the
         differentiable fp32 path (_FieldTrainFn) and returns density / color / fields_penalty."""
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            ray_dir = L.require_cuda_f32(ray_dir, "ray_dir")
-            ray_orig = L.require_cuda_f32(ray_orig, "ray_orig")
-            dists = L.require_cuda_f32(dists, "dists")
-            flat = [t for l in self._ordered_layers() for t in (l.weight, l.bias)]
-            d, c, pnl = _FieldTrainFn.apply(self, ray_dir, ray_orig, dists, sampling_type, ray_radius, *flat)
-            return {"density": d, "color": c, "fields_penalty": pnl}
         ray_dir = L.require_cuda_f32(ray_dir, "ray_dir")
         ray_orig = L.require_cuda_f32(ray_orig, "ray_orig")
         dists = L.require_cuda_f32(dists, "dists")
+        if self._wants_grad():
+            d, c, pnl = _FieldTrainFn.apply(self, ray_dir, ray_orig, dists, sampling_type, ray_radius,
+                                            *self._param_tensors())
+            return {"density": d, "color": c, "fields_penalty": pnl}
         B, S = dists.shape
         device = dists.device
         out = {
@@ -532,20 +517,13 @@ class NeDDF(BaseNeuralField):
             out["aux_grad"] = torch.empty(B, S, device=device, dtype=torch.float32)
         h = self._field(device)
         st = self._state_struct()
-        prof = self._profile_events
-        if prof is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record(torch.cuda.current_stream(device))
-        with torch.cuda.device(device):
+        with self._profiled(device, B * S), torch.cuda.device(device):
             L.check(L.lib().neddf_field_forward_rays(
                 h, C.byref(st), L.ptr(ray_dir), L.ptr(ray_orig), L.ptr(dists), B, S, L.SAMPLING_IDS[sampling_type],
                 float(ray_radius), L.ptr(out.get("distance")), L.ptr(out["density"]), L.ptr(out["color"]),
                 L.ptr(out.get("fields_penalty")), L.ptr(out.get("aux_grad")),
                 L.OUT_FULL if need_penalty else L.OUT_EVAL, self._engine_id(), L.stream_ptr(device)),
                 "field_forward_rays")
-        if prof is not None:
-            e1.record(torch.cuda.current_stream(device))
-            prof.append((e0, e1, B * S))
         return out
 
     def forward_rays_segment(self, ray_dir: Tensor, ray_orig: Tensor, dists: Tensor, sampling_type: str, ray_radius: float,
@@ -558,18 +536,12 @@ class NeDDF(BaseNeuralField):
         device = dists.device
         h = self._field(device)
         st = self._state_struct()
-        prof = self._profile_events
-        if prof is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record(torch.cuda.current_stream(device))
-        with torch.cuda.device(device):
+        # the executed count lives on the device (NeRFRender.termination_stats): no n_evaluations
+        with self._profiled(device, None), torch.cuda.device(device):
             L.check(L.lib().neddf_field_forward_rays_segment(
                 h, C.byref(st), L.ptr(ray_dir), L.ptr(ray_orig), L.ptr(dists), B, E, L.SAMPLING_IDS[sampling_type],
                 float(ray_radius), int(edge0), int(seg_len), L.ptr(ray_index), L.ptr(n_active), L.ptr(density),
                 L.ptr(color), self._engine_id(), L.stream_ptr(device)), "field_forward_rays_segment")
-        if prof is not None:
-            e1.record(torch.cuda.current_stream(device))
-            prof.append((e0, e1, None))  # the executed count lives on the device (NeRFRender.termination_stats)
 
     def check_engine_status(self) -> None:
         """Read-and-clear the engine's device status word (one sync).  Raises if the tensor-core

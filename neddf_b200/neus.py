@@ -23,6 +23,7 @@ import torch
 from torch import Tensor, nn
 
 from . import _lib as L
+from ._host import KernelHandle, WeightGrad
 from .network import BaseNeuralField
 from .ray import Sampling
 
@@ -86,32 +87,12 @@ class _NeusTrainFn(torch.autograd.Function):
                 L.check(lib.neddf_neus_train_backward(
                     h, L.ptr(a), L.ptr(b), n, L.ptr(g_sdf), L.ptr(g_density), L.ptr(g_color), L.ptr(g_normal), bufs, stream),
                     "neus_train_backward")
-            ws = getattr(net, "_wgrad_ws", None)
-            if ws is None or ws.device != device:
-                ws = torch.empty(int(lib.neddf_wgrad_workspace_bytes()) // 4, **f32)
-                net._wgrad_ws = ws
-
-            def wgrad_into(out, row0, A, lda, ka, Bm, rows):
-                """out[row0 : row0 + ka, :256] = A[:, :ka]^T Bm (rows x 256), 128 columns of A at a time."""
-                for c0 in range(0, ka, 128):
-                    kk = min(128, ka - c0)
-                    L.check(lib.neddf_wgrad(L.ptr(A), lda, c0, kk, L.ptr(Bm), W, rows,
-                                            C.c_void_p(out.data_ptr() + 4 * (row0 + c0) * out.shape[1]), out.shape[1], W,
-                                            L.ptr(ws), stream), "wgrad")
-
-            def colsum(Gm, stride):
-                out = torch.empty(W, **f32)
-                L.check(lib.neddf_colsum_value_rows(L.ptr(Gm), n, stride, L.ptr(out), L.ptr(ws), stream), "colsum")
-                return out
+            wg = WeightGrad(net, device, n)
 
             def layer_grad(parts, Gm, rows, stride):
                 """d weight [out, in] and d bias of a layer with inputs `parts` (A, columns) over `rows` rows."""
-                gWt = torch.empty(sum(k for _, k in parts), W, **f32)
-                row0 = 0
-                for Xp, k_in in parts:
-                    wgrad_into(gWt, row0, Xp, k_in, k_in, Gm, rows)
-                    row0 += k_in
-                return [gWt.t().contiguous(), colsum(Gm, stride)]
+                gWt, gb = wg.layer(parts, Gm, rows, stride)
+                return [gWt.t().contiguous(), gb]
 
             grads = []
             for l in range(Ls):  # layers_sdf.l over the 4 rows of every sample: in_0 = E4, in_l = [XS_{l-1} | E4 if skip]
@@ -120,8 +101,8 @@ class _NeusTrainFn(torch.autograd.Function):
             grads += layer_grad([(XC0, n_x), (FO, W)], GC[0], n, W)  # layers_col.0: [pos | dir PE | normal | F]
             for l in range(1, Lc):
                 grads += layer_grad([(XC[l - 1], W)], GC[l], n, W)
-            gh = torch.empty(3, W, **f32)  # the 3-channel output layer: GH^T h_{Lc-1}, already [out, in]
-            wgrad_into(gh, 0, GH, 3, 3, XC[Lc - 1], n)
+            gh = wg.empty(3, W)  # the 3-channel output layer: GH^T h_{Lc-1}, already [out, in]
+            wg.into(gh, 0, GH, 3, 3, XC[Lc - 1], n)
             grads += [gh, GH.sum(0), GV.sum()]
         return (None,) * 7 + tuple(grads)
 
@@ -129,6 +110,11 @@ class _NeusTrainFn(torch.autograd.Function):
 class NeuS(BaseNeuralField):
     # sdf grows outward; density is a bump around the surface, not monotone across it, so it has no outside
     _MESH_VIEW_SIGN = {"sdf": -1.0}
+    _HANDLES = (KernelHandle("neddf_neus"), KernelHandle("neddf_neus_train", "_train"))
+    _GRAD_REFUSAL = (
+        "neddf_b200.NeuS is forward-only on the CUDA path by default: wrap the call in torch.no_grad() / use "
+        "render_image, or opt in to the training backward kernel (csrc/neus_train.cu) with "
+        "net.training_kernels = True or NEDDF_NEUS_TRAIN=1")
 
     def __init__(
         self,
@@ -168,15 +154,8 @@ class NeuS(BaseNeuralField):
         self.variance = nn.Parameter(torch.tensor(init_variance))
         # kernel-side state
         self.engine = "fp32"  # the only engine of this variant; NeRFRender.set_engine may overwrite the attribute
-        self._handle = None
-        self._handle_device = None
-        self._packed_key = None
-        self._profile_events = None
         # training backward (csrc/neus_train.cu): opt-in, the default stays the forward-only refusal
         self.training_kernels = os.environ.get("NEDDF_NEUS_TRAIN", "0") not in ("", "0")
-        self._train_handle = None
-        self._train_handle_device = None
-        self._train_packed_key = None
 
     # ------------------------------------------------------------------ kernel plumbing --
     def _ordered_layers(self) -> List[nn.Linear]:
@@ -188,115 +167,11 @@ class NeuS(BaseNeuralField):
         c.sdf_layer_count, c.sdf_layer_width = self.sdf_layer_count, self.sdf_layer_width
         c.col_layer_count, c.col_layer_width = self.col_layer_count, self.col_layer_width
         c.activation_type = L.ACT_IDS[self.activation_type]
-        if len(self.skips) > L.MAX_SKIPS:
-            raise NotImplementedError("neddf_b200: more than 8 skip connections")
-        c.n_skips = len(self.skips)
-        for i, s in enumerate(self.skips):
-            c.skips[i] = s
-        return c
+        return self._fill_skips(c)
 
     def _param_tensors(self) -> List[Tensor]:
-        return [p for l in self._ordered_layers() for p in (l.weight, l.bias)] + [self.variance]
-
-    def _train_field(self, device: torch.device):
-        """Handle of the training-backward kernel (forward + transposed weight packs), re-packed when a parameter changed
-        (keyed on the tensors' version counters, like _field)."""
-        lib = L.lib()
-        if self._train_handle is None or self._train_handle_device != device:
-            self._release_train()
-            h = C.c_void_p()
-            with torch.cuda.device(device):
-                cfg = self._config_struct()
-                L.check(lib.neddf_neus_train_create(C.byref(cfg), C.byref(h)), "neus_train_create")
-            self._train_handle, self._train_handle_device = h, device
-        layers = self._ordered_layers()
-        key = tuple((p.data_ptr(), p._version) for p in self._param_tensors())
-        if key != self._train_packed_key:
-            n = len(layers)
-            ws = (C.c_void_p * n)(*[l.weight.data_ptr() for l in layers])
-            bs = (C.c_void_p * n)(*[l.bias.data_ptr() for l in layers])
-            with torch.cuda.device(device):
-                L.check(lib.neddf_neus_train_set_weights(self._train_handle, ws, bs, n, L.ptr(self.variance),
-                                                         L.stream_ptr(device)), "neus_train_set_weights")
-            self._train_packed_key = key
-        return self._train_handle
-
-    def _release_train(self) -> None:
-        if self._train_handle is not None:
-            L.lib().neddf_neus_train_destroy(self._train_handle)
-        self._train_handle, self._train_handle_device, self._train_packed_key = None, None, None
-
-    def _release(self) -> None:
-        if self._handle is not None:
-            L.lib().neddf_neus_destroy(self._handle)
-        self._handle, self._handle_device, self._packed_key = None, None, None
-        if getattr(self, "_train_handle", None) is not None:
-            self._release_train()
-
-    def __del__(self):
-        try:
-            self._release()
-        except Exception:  # interpreter shutdown
-            pass
-
-    def _field(self, device: torch.device):
-        lib = L.lib()
-        if device.type != "cuda":
-            raise RuntimeError("neddf_b200.NeuS runs on CUDA devices only: move the module with .to('cuda') "
-                               "(the hot path has no CPU implementation)")
-        if self._handle is None or self._handle_device != device:
-            self._release()
-            h = C.c_void_p()
-            with torch.cuda.device(device):
-                cfg = self._config_struct()
-                L.check(lib.neddf_neus_create(C.byref(cfg), C.byref(h)), "neus_create")
-            self._handle, self._handle_device = h, device
-        layers = self._ordered_layers()
-        tensors = [p for l in layers for p in (l.weight, l.bias)] + [self.variance]
-        key = tuple((p.data_ptr(), p._version) for p in tensors)
-        if key != self._packed_key:
-            for p in tensors:
-                if p.dtype != torch.float32 or not p.is_contiguous() or p.device != device:
-                    raise RuntimeError("neddf_b200: parameters must be contiguous fp32 tensors on the module's device")
-            n = len(layers)
-            ws = (C.c_void_p * n)(*[l.weight.data_ptr() for l in layers])
-            bs = (C.c_void_p * n)(*[l.bias.data_ptr() for l in layers])
-            with torch.cuda.device(device):
-                L.check(lib.neddf_neus_set_weights(self._handle, ws, bs, n, L.ptr(self.variance), L.stream_ptr(device)),
-                        "neus_set_weights")
-            self._packed_key = key
-        return self._handle
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        self._packed_key = None  # .to()/.cuda() replaced the parameter storage
-        self._train_packed_key = None
-        return r
-
-    def invalidate(self) -> None:
-        self._packed_key = None
-        self._train_packed_key = None
-
-    def __getstate__(self):
-        d = self.__dict__.copy()
-        d["_handle"], d["_handle_device"], d["_packed_key"], d["_profile_events"] = None, None, None, None
-        d["_train_handle"], d["_train_handle_device"], d["_train_packed_key"] = None, None, None
-        d.pop("_wgrad_ws", None)
-        return d
-
-    def check_engine_status(self) -> None:
-        """(fp32 kernel: no range checks to report)"""
-
-    def _wants_grad(self) -> bool:
-        """Autograd is recording and some parameter is trainable.  Without the opt-in that is refused."""
-        if not (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())):
-            return False
-        if not self.training_kernels:
-            raise NotImplementedError(
-                "neddf_b200.NeuS is forward-only on the CUDA path by default: wrap the call in torch.no_grad() / use "
-                "render_image, or opt in to the training backward kernel (csrc/neus_train.cu) with "
-                "net.training_kernels = True or NEDDF_NEUS_TRAIN=1")
-        return True
+        """The layers' weights and biases, then the variance (packed too: the extra argument of the set_weights calls)."""
+        return super()._param_tensors() + [self.variance]
 
     def _launch_forward(self, a: Tensor, b: Tensor, c, sampling_type, ray_radius: float, with_normal: bool) -> Dict[str, Tensor]:
         """The inference kernel on rays (sampling_type given) or explicit samples; called under no_grad."""
@@ -353,16 +228,9 @@ class NeuS(BaseNeuralField):
         device = dists.device
         out = self._outputs(B, S, device, with_normal)
         h = self._field(device)
-        prof = self._profile_events
-        if prof is not None:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record(torch.cuda.current_stream(device))
-        with torch.cuda.device(device):
+        with self._profiled(device, B * S), torch.cuda.device(device):
             L.check(L.lib().neddf_neus_forward_rays(h, L.ptr(ray_dir), L.ptr(ray_orig), L.ptr(dists), B, S,
                                                     L.SAMPLING_IDS[sampling_type], float(ray_radius), L.ptr(out["sdf"]),
                                                     L.ptr(out["density"]), L.ptr(out["color"]), L.ptr(out.get("normal")),
                                                     L.stream_ptr(device)), "neus_forward_rays")
-        if prof is not None:
-            e1.record(torch.cuda.current_stream(device))
-            prof.append((e0, e1, B * S))
         return out

@@ -2,10 +2,10 @@
 
 The reference steps ``torch.optim.Adam`` over ``neural_render.get_parameters_list()`` (nerf_trainer.py:38-42,
 129); the CUDA field kernels then need their packed copies of the weights refreshed.  ``FusedAdam`` does the
-update of every tensor of a network in ONE launch (``neddf_field_adam_step``) and re-packs on the same stream, so
-a training step has no per-tensor optimiser kernels and no separate "parameters changed" detection.
-It is a ``torch.optim.Optimizer`` (param_groups, lr schedulers work); parameters that do not belong to a
-neddf_b200.NeDDF module are stepped by the same kernel without a re-pack.
+update of every tensor of a network in ONE launch (``neddf_field_adam_step``) and, for a NeDDF, re-packs on the same
+stream, so a training step has no per-tensor optimiser kernels and no separate "parameters changed" detection.
+It is a ``torch.optim.Optimizer`` (param_groups, lr schedulers work); parameters that do not belong to one of its
+networks are stepped by the same kernel without a re-pack.
 """
 import ctypes as C
 from typing import Iterable, List
@@ -13,13 +13,15 @@ from typing import Iterable, List
 import torch
 
 from . import _lib as L
+from .network import NeDDF
 
 
 class FusedAdam(torch.optim.Optimizer):
     def __init__(self, params: Iterable, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 0.0, networks: Iterable = ()) -> None:
-        """``networks``: the neddf_b200.NeDDF modules whose parameters are in ``params`` (their packed weights
-        are refreshed by the step); ``FusedAdam.for_render(render, ...)`` fills both."""
+        """``networks``: the neddf_b200 field networks whose parameters are in ``params``.  A NeDDF's packed weights
+        are refreshed by the step itself; a NeRF or NeuS re-packs on its next call.  ``FusedAdam.for_render(render,
+        ...)`` fills both."""
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
         self._networks: List = list({id(n): n for n in networks}.values())
         self._steps = 0
@@ -41,7 +43,7 @@ class FusedAdam(torch.optim.Optimizer):
         loss = closure() if closure is not None else None
         self._steps += 1
         lib = L.lib()
-        done = set()
+        done, repacked = set(), set()
         for group in self.param_groups:
             lr, (b1, b2), eps, wd = group["lr"], group["betas"], group["eps"], group["weight_decay"]
             in_group = {id(p) for p in group["params"]}
@@ -60,13 +62,12 @@ class FusedAdam(torch.optim.Optimizer):
                 n = len(ps)
                 grads = [p.grad.contiguous() for p in ps]
                 st = [self._state(p) for p in ps]
-                arr = lambda ts: (C.c_void_p * n)(*[t.data_ptr() for t in ts])  # noqa: E731
-                numel = (C.c_int64 * n)(*[p.numel() for p in ps])
-                handle = net._field(device) if net is not None else None
+                # the step re-packs a neddf_field_t* behind the update: only a NeDDF has one.  Without a handle the
+                # launch takes at most 64 tensors.
+                handle = net._field(device) if isinstance(net, NeDDF) else None
                 with torch.cuda.device(device):
-                    for i in range(0, n, 64) if net is None else (0,):
-                        m = n if net is not None else min(64, n - i)
-                        sl = slice(i, i + m)
+                    for sl in [slice(i, i + 64) for i in range(0, n, 64)] if handle is None else [slice(0, n)]:
+                        m = len(ps[sl])
                         L.check(lib.neddf_field_adam_step(
                             handle, (C.c_void_p * m)(*[t.data_ptr() for t in ps[sl]]),
                             (C.c_void_p * m)(*[t.data_ptr() for t in grads[sl]]),
@@ -74,5 +75,9 @@ class FusedAdam(torch.optim.Optimizer):
                             (C.c_void_p * m)(*[s["exp_avg_sq"].data_ptr() for s in st[sl]]),
                             (C.c_int64 * m)(*[p.numel() for p in ps[sl]]), m, float(lr), float(b1), float(b2), float(eps),
                             float(wd), self._steps, L.stream_ptr(device)), "adam_step")
-                del arr, numel
+                if handle is not None:
+                    repacked.add(id(net))
+        for net in self._networks:  # the kernel wrote parameters without bumping their version counters
+            if id(net) not in repacked:
+                net.invalidate()
         return loss
