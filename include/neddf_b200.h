@@ -500,6 +500,47 @@ int32_t neddf_mc_normals(const float* d_volume, int32_t n0, int32_t n1, int32_t 
                          const void* d_workspace, const float* d_vertices, const int64_t* d_faces, float* d_normals,
                          void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Sphere tracing of a level set (csrc/surface.cu; no reference function is replaced - the reference shows its
+ * surfaces only through volumetric renders and its Open3D visualiser).  Per ray g(t) = field(o + t d) - level;
+ * stepping t += g is safe where |dD/dt| <= 1, which NeDDF trains (constraints_dDdt, neddf/network/neddf.py:271).
+ * State machine, per ray, one field evaluation per step (every float operation rounded on its own):
+ *   MARCH   g >= EPS: lo = t, t += g, MISS if t > far;  0 <= g < EPS: HIT at t;  g < 0: BISECT [lo, t]
+ *           (g < 0 at the first evaluation: MISS - the ray starts inside the level set)
+ *   BISECT  8 evaluations at lo + (hi - lo) * 0.5 keeping g(lo) >= 0 > g(hi); then HIT at lo
+ *   a ray that has spent max_steps evaluations without a hit is a MISS; a MISS sets t = far.
+ * Per-ray arrays: d_t, d_t_lo, d_t_hi fp32 [n], d_state, d_steps int32 [n].  The live list (int32 ray ids) and the
+ * packed samples d_pos / d_dir [n_live, 3] it evaluates next come in any order; outputs do not depend on it.
+ *   neddf_trace_init       t = lo = hi = near, state MARCH, steps 0, live = 0..n-1, samples at t = near.
+ *   neddf_trace_step       d_values [n_live]: the field at the samples of d_live; writes the next live list, its count
+ *                          (d_count_next, int32 [1], zeroed here) and its samples.
+ *   neddf_trace_hits       the HIT rays: list, count (int32 [1]), hit points o + t d and directions, packed.
+ *   neddf_trace_fd_points  6 central-difference points per hit (x+h, x-h, y+h, y-h, z+h, z-h; h = 1e-4) with the hit's
+ *                          direction, [6 n_hits, 3].
+ *   neddf_trace_fd_normals d_values [6 n_hits] at those points -> unit normals (toward increasing value; 0 for a zero
+ *                          difference) written to d_normal [ray id, 3].
+ * ------------------------------------------------------------------------------------------------ */
+#define NEDDF_TRACE_MARCH 0
+#define NEDDF_TRACE_BISECT 1 /* 1..8: halvings done before the pending evaluation, plus one */
+#define NEDDF_TRACE_HIT 16
+#define NEDDF_TRACE_MISS 17
+#define NEDDF_TRACE_EPS 1e-4f
+#define NEDDF_TRACE_FD_H 1e-4f
+int32_t neddf_trace_init(const float* d_ray_dir, const float* d_ray_orig, int64_t n_rays, float near, float* d_t,
+                         float* d_t_lo, float* d_t_hi, int32_t* d_state, int32_t* d_steps, int32_t* d_live,
+                         float* d_pos, float* d_dir, void* stream);
+int32_t neddf_trace_step(const float* d_values, const int32_t* d_live, int64_t n_live, const float* d_ray_dir,
+                         const float* d_ray_orig, float far, float level, int32_t max_steps, float* d_t, float* d_t_lo,
+                         float* d_t_hi, int32_t* d_state, int32_t* d_steps, int32_t* d_live_next,
+                         int32_t* d_count_next, float* d_pos, float* d_dir, void* stream);
+int32_t neddf_trace_hits(const float* d_ray_dir, const float* d_ray_orig, int64_t n_rays, const float* d_t,
+                         const int32_t* d_state, int32_t* d_hits, int32_t* d_count, float* d_pos, float* d_dir,
+                         void* stream);
+int32_t neddf_trace_fd_points(const float* d_hit_pos, const float* d_hit_dir, int64_t n_hits, float* d_points,
+                              float* d_dirs, void* stream);
+int32_t neddf_trace_fd_normals(const float* d_values, const float* d_hit_pos, const int32_t* d_hits, int64_t n_hits,
+                               float* d_normal, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -125,7 +125,16 @@ _SIGNATURES = {
     "neddf_mc_count": (_I32, [_P, _I32, _I32, _I32, _F, _P, _P, _P]),
     "neddf_mc_emit": (_I32, [_P, _I32, _I32, _I32, _F, _P, _P, _P, _P]),
     "neddf_mc_normals": (_I32, [_P, _I32, _I32, _I32, _F, _P, _P, _P, _P, _P]),
+    "neddf_trace_init": (_I32, [_P, _P, _I64, _F] + [_P] * 8 + [_P]),
+    "neddf_trace_step": (_I32, [_P, _P, _I64, _P, _P, _F, _F, _I32] + [_P] * 9 + [_P]),
+    "neddf_trace_hits": (_I32, [_P, _P, _I64, _P, _P, _P, _P, _P, _P, _P]),
+    "neddf_trace_fd_points": (_I32, [_P, _P, _I64, _P, _P, _P]),
+    "neddf_trace_fd_normals": (_I32, [_P, _P, _P, _I64, _P, _P]),
 }
+
+# csrc/surface.cu (include/neddf_b200.h NEDDF_TRACE_*)
+TRACE_MARCH, TRACE_BISECT, TRACE_HIT, TRACE_MISS = 0, 1, 16, 17
+TRACE_EPS, TRACE_FD_H, TRACE_BISECTIONS = 1e-4, 1e-4, 8
 
 _lib = None
 

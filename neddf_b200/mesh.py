@@ -163,15 +163,9 @@ def read_ply(path: str, attributes: bool = False):
     return out
 
 
-# network class name -> (field, threshold); NeRF has no canonical level
-DEFAULTS = {"NeDDF": ("distance", 0.0275), "NeuS": ("sdf", 0.0), "NeRF": ("density", None)}
-
-
-def mesh_run(run_dir: str, epoch: int = 2000, resolution: int = 64, threshold: Optional[float] = None,
-             field: Optional[str] = None, out: Optional[str] = None, cube_range: float = 1.1,
-             device: str = "cuda:0", color: bool = False) -> str:
-    """The headless half of the reference visualiser's main / generate_mesh: returns the written PLY's path.
-    ``color=True`` also writes the vertex normals and colours of ``extract_mesh(..., with_color=True)``."""
+def load_run(run_dir: str, epoch: int = 2000, device: str = "cuda:0"):
+    """The NeRFRender of a training run: ``RUN_DIR/.hydra/config.yaml`` with ``RUN_DIR/models/model_{epoch:05}.pth``
+    loaded, on ``device``."""
     import yaml
 
     from .render import NeRFRender
@@ -183,8 +177,18 @@ def mesh_run(run_dir: str, epoch: int = 2000, resolution: int = 64, threshold: O
     state = torch.load(os.path.join(run_dir, "models", f"model_{epoch:05}.pth"), map_location="cpu")
     render.load_state_dict(state)
     render.to(torch.device(device))
-    net = render.get_network()
-    default_field, default_thr = DEFAULTS[type(net).__name__]
+    return render
+
+
+def mesh_run(run_dir: str, epoch: int = 2000, resolution: int = 64, threshold: Optional[float] = None,
+             field: Optional[str] = None, out: Optional[str] = None, cube_range: float = 1.1,
+             device: str = "cuda:0", color: bool = False) -> str:
+    """The headless half of the reference visualiser's main / generate_mesh: returns the written PLY's path.
+    ``color=True`` also writes the vertex normals and colours of ``extract_mesh(..., with_color=True)``."""
+    from .network import LEVEL_DEFAULTS
+
+    net = load_run(run_dir, epoch, device).get_network()
+    default_field, default_thr = LEVEL_DEFAULTS[type(net).__name__]
     field = field or default_field
     if threshold is None:
         threshold = default_thr

@@ -163,6 +163,12 @@ class _FieldTrainFn(torch.autograd.Function):
         return (None, None, None, None, None, None) + tuple(grads)
 
 
+# network class name -> (field, level) of its surface: the level set ``extract_mesh`` meshes by default (``python -m
+# neddf_b200.mesh``) and ``trace_surface`` traces (``NeRFRender.render_surface``).  NeDDF: the reference visualiser's
+# iso-level of the distance field; NeuS: the SDF's zero set; NeRF has no canonical level.
+LEVEL_DEFAULTS = {"NeDDF": ("distance", 0.0275), "NeuS": ("sdf", 0.0), "NeRF": ("density", None)}
+
+
 class EngineRangeError(FloatingPointError):
     """The tensor-core engine left fp16 range under engine "auto"; the network has switched itself to the fp32 engine
     and the caller (NeRFRender) re-runs the call.  Explicit engines ("tc", "tc2") raise plain FloatingPointError."""
@@ -348,6 +354,112 @@ class BaseNeuralField(nn.Module):
                 colors = self._vertex_colors(world, view_dir)
         return world, faces, normals, colors
 
+    # the field whose values sphere tracing may step by (a distance or an SDF); None: the network cannot be traced
+    _TRACE_FIELD: Optional[str] = None
+
+    def surface_level(self, level: Optional[float] = None) -> float:
+        """``level``, or the network's default surface level (``LEVEL_DEFAULTS``).  ValueError for a network without a
+        distance field to trace (NeRF)."""
+        if self._TRACE_FIELD is None:
+            raise ValueError(f"{type(self).__name__} has no distance field: its surface cannot be sphere-traced")
+        if level is None:
+            level = LEVEL_DEFAULTS[type(self).__name__][1]
+        level = float(level)
+        if not np.isfinite(level) or abs(level) > float(np.finfo(np.float32).max):
+            raise ValueError(f"trace_surface: level must be a finite fp32 value, got {level!r}")
+        return level
+
+    @staticmethod
+    def _check_trace_args(near: float, far: float, max_steps: int) -> None:
+        if not isinstance(max_steps, (int, np.integer)) or isinstance(max_steps, bool) or not 1 <= max_steps < 2 ** 31:
+            raise ValueError(f"trace_surface: max_steps must be an integer >= 1, got {max_steps!r}")
+        if not (np.isfinite(near) and np.isfinite(far) and 0.0 <= near < far):
+            raise ValueError(f"trace_surface: need finite 0 <= near < far, got near={near!r}, far={far!r}")
+
+    def trace_surface(self, ray_dir: Tensor, ray_orig: Tensor, near: float, far: float, level: float,
+                      max_steps: int = 128) -> Dict[str, Tensor]:
+        """First hit of the level set ``field == level`` along each ray by sphere tracing (csrc/surface.cu), under
+        no_grad.  ``ray_dir`` (unit) / ``ray_orig`` [n,3] on the module's device.  Returns flat per-ray tensors:
+        ``depth`` [n] (t of the hit; ``far`` on a miss), ``hit`` [n] bool, ``normal`` [n,3] (unit, toward increasing
+        value; 0 on a miss), ``color`` [n,3] (the field's colour at the hit seen along the ray; 0 on a miss) and
+        ``steps`` [n] int32 (field evaluations spent on the ray, normals and colour not counted).
+
+        g(t) = field(o + t d) - level is evaluated through ``forward`` with point samples, zero variance and view
+        direction d in the module's current ``set_iter`` state, as ``extract_mesh`` evaluates its grid.  From t = near:
+        g >= EPS (1e-4) steps t += g (beyond far: miss), 0 <= g < EPS is a hit, g < 0 bisects the last step 8 times
+        and hits at the near end of the bracket, so every hit has g >= 0.  g < 0 at t = near (the ray starts inside)
+        and max_steps evaluations without a hit are misses.  One host read of the live count (4 bytes) per iteration:
+        the point-query forwards take their sample count from the host.  Under engine "auto" the engine status is
+        read once at the end; if the tensor-core engine left fp16 range the trace is run again on the fp32 engine."""
+        level = self.surface_level(level)
+        near, far = float(near), float(far)
+        self._check_trace_args(near, far, max_steps)
+        ray_dir = L.require_cuda_f32(ray_dir, "ray_dir")
+        ray_orig = L.require_cuda_f32(ray_orig, "ray_orig")
+        if ray_dir.dim() != 2 or ray_dir.shape[1] != 3 or ray_orig.shape != ray_dir.shape:
+            raise ValueError(f"trace_surface: rays must be [n,3], got {tuple(ray_dir.shape)} / {tuple(ray_orig.shape)}")
+        out = self._trace(ray_dir, ray_orig, near, far, level, int(max_steps))
+        if getattr(self, "engine", None) == "auto":
+            try:
+                self.check_engine_status()
+            except EngineRangeError as e:  # engine "auto" left fp16 range: trace again on the fp32 engine
+                warnings.warn(str(e), RuntimeWarning)
+                out = self._trace(ray_dir, ray_orig, near, far, level, int(max_steps))
+        return out
+
+    def _trace_values(self, pos: Tensor, dirs: Tensor) -> Tensor:
+        """``forward`` of packed samples [m,3] with zero variance -> the traced field [m]."""
+        p = pos[None]
+        return self.forward(Sampling(p, dirs[None], torch.zeros_like(p)))[self._TRACE_FIELD].reshape(-1)
+
+    def _trace(self, ray_dir: Tensor, ray_orig: Tensor, near: float, far: float, level: float,
+               max_steps: int) -> Dict[str, Tensor]:
+        lib = L.lib()
+        n = ray_dir.shape[0]
+        device = ray_dir.device
+        f32, i32 = dict(device=device, dtype=torch.float32), dict(device=device, dtype=torch.int32)
+        t, lo, hi = (torch.empty(n, **f32) for _ in range(3))
+        state, steps, count = torch.empty(n, **i32), torch.empty(n, **i32), torch.empty(1, **i32)
+        live = [torch.empty(n, **i32), torch.empty(n, **i32)]
+        pos, dirs = torch.empty(n, 3, **f32), torch.empty(n, 3, **f32)
+        normal, color = torch.zeros(n, 3, **f32), torch.zeros(n, 3, **f32)
+        with torch.no_grad(), torch.cuda.device(device):
+            stream = L.stream_ptr(device)
+            L.check(lib.neddf_trace_init(L.ptr(ray_dir), L.ptr(ray_orig), n, near, L.ptr(t), L.ptr(lo), L.ptr(hi),
+                                         L.ptr(state), L.ptr(steps), L.ptr(live[0]), L.ptr(pos), L.ptr(dirs), stream),
+                    "trace_init")
+            n_live, k = n, 0
+            while n_live:  # every live ray spends one evaluation per pass, so at most max_steps passes
+                values = self._trace_values(pos[:n_live], dirs[:n_live])
+                L.check(lib.neddf_trace_step(L.ptr(values), L.ptr(live[k]), n_live, L.ptr(ray_dir), L.ptr(ray_orig),
+                                             far, level, max_steps, L.ptr(t), L.ptr(lo), L.ptr(hi), L.ptr(state),
+                                             L.ptr(steps), L.ptr(live[1 - k]), L.ptr(count), L.ptr(pos), L.ptr(dirs),
+                                             stream), "trace_step")
+                k = 1 - k
+                n_live = int(count.item())
+            hits = live[k]
+            L.check(lib.neddf_trace_hits(L.ptr(ray_dir), L.ptr(ray_orig), n, L.ptr(t), L.ptr(state), L.ptr(hits),
+                                         L.ptr(count), L.ptr(pos), L.ptr(dirs), stream), "trace_hits")
+            n_hit = int(count.item())
+            if n_hit:
+                self._shade_hits(hits[:n_hit], pos[:n_hit], dirs[:n_hit], normal, color)
+        return {"depth": t, "hit": state == L.TRACE_HIT, "normal": normal, "color": color, "steps": steps}
+
+    def _shade_hits(self, hits: Tensor, pos: Tensor, dirs: Tensor, normal: Tensor, color: Tensor) -> None:
+        """Normals and colours of the hit rays ``hits`` (packed hit points ``pos``, ray directions ``dirs``), stored by
+        ray id.  Normals by central differences of the traced field (6 points per hit, h = 1e-4): the distance
+        Jacobian the NeDDF kernels carry is not one of their outputs."""
+        lib = L.lib()
+        m = hits.shape[0]
+        device = pos.device
+        pts, pdirs = torch.empty(6 * m, 3, device=device), torch.empty(6 * m, 3, device=device)
+        stream = L.stream_ptr(device)
+        L.check(lib.neddf_trace_fd_points(L.ptr(pos), L.ptr(dirs), m, L.ptr(pts), L.ptr(pdirs), stream), "trace_fd_points")
+        values = self._trace_values(pts, pdirs)
+        L.check(lib.neddf_trace_fd_normals(L.ptr(values), L.ptr(pos), L.ptr(hits), m, L.ptr(normal), stream),
+                "trace_fd_normals")
+        color.index_copy_(0, hits.long(), self._vertex_colors(pos, dirs))
+
     def _vertex_colors(self, points: Tensor, view_dir: Tensor, chunk: int = 65536) -> Tensor:
         """``forward(Sampling(points, view_dir, 0))["color"]`` [V,3] in chunks, with no host synchronisation."""
         with torch.set_grad_enabled(False):
@@ -364,6 +476,7 @@ class NeDDF(BaseNeuralField):
 
     _MESH_VIEW_SIGN = {"distance": -1.0, "density": 1.0}  # distance grows outward, density inward
     _HANDLES = (KernelHandle("neddf_field"),)
+    _TRACE_FIELD = "distance"
 
     def __init__(
         self,

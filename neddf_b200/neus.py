@@ -28,6 +28,11 @@ from .network import BaseNeuralField
 from .ray import Sampling
 
 
+def unit_normals(g: Tensor) -> Tensor:
+    """The SDF gradient [m,3] as unit normals (``F.normalize``: a zero gradient stays 0)."""
+    return torch.nn.functional.normalize(g, dim=1)
+
+
 class _NeusTrainFn(torch.autograd.Function):
     """NeuS.forward under autograd.  forward: the inference kernel (neddf_neus_forward[_rays]); backward:
     neddf_neus_train_backward[_rays] (recomputes the forward per tile, leaves the layer inputs and pre-activation
@@ -110,6 +115,7 @@ class _NeusTrainFn(torch.autograd.Function):
 class NeuS(BaseNeuralField):
     # sdf grows outward; density is a bump around the surface, not monotone across it, so it has no outside
     _MESH_VIEW_SIGN = {"sdf": -1.0}
+    _TRACE_FIELD = "sdf"
     _HANDLES = (KernelHandle("neddf_neus"), KernelHandle("neddf_neus_train", "_train"))
     _GRAD_REFUSAL = (
         "neddf_b200.NeuS is forward-only on the CUDA path by default: wrap the call in torch.no_grad() / use "
@@ -185,6 +191,15 @@ class NeuS(BaseNeuralField):
         if with_normal:
             out["normal"] = res[3]
         return out
+
+    def _shade_hits(self, hits: Tensor, pos: Tensor, dirs: Tensor, normal: Tensor, color: Tensor) -> None:
+        """The exact normal of ``forward(with_normal=True)``, normalised (``unit_normals``), and the colour of the same
+        call, stored by ray id."""
+        p = pos[None]
+        out = self.forward(Sampling(p, dirs[None], p), with_normal=True)
+        idx = hits.long()
+        normal.index_copy_(0, idx, unit_normals(out["normal"].reshape(-1, 3)))
+        color.index_copy_(0, idx, out["color"].reshape(-1, 3))
 
     @staticmethod
     def _outputs(B: int, S: int, device, with_normal: bool) -> Dict[str, Tensor]:

@@ -494,6 +494,36 @@ class NeRFRender(BaseNeuralRender):
                 self.check_status()
         return {k: v.reshape(h, w, -1) for k, v in flat.items()}
 
+    def render_surface(self, width: int, height: int, camera, downsampling: int = 1, level: Optional[float] = None,
+                       max_steps: int = 128) -> Dict[str, Tensor]:
+        """The first surface hit of every pixel of ``render_image``'s grid (same rays, ``neddf_make_image_rays``),
+        sphere-traced from ``dist_near`` to ``dist_far`` on the level set ``field == level`` of ``get_network()``
+        (``BaseNeuralField.trace_surface``; ``level=None``: the network's default, ``network.LEVEL_DEFAULTS``).
+        Images [h, w, C] with h, w = height // downsampling, width // downsampling: ``depth`` [h,w,1] (t along the
+        unit ray direction, the unit of the volumetric depth; ``dist_far`` on a miss), ``hit`` [h,w,1] bool,
+        ``normal`` [h,w,3] (unit, world frame, toward increasing value; 0 on a miss), ``color`` [h,w,3] (0 on a miss),
+        ``steps`` [h,w,1] int32.  The whole frame is traced in one sequence.  NeRF has no distance field: ValueError."""
+        width, height, downsampling = (int(v) for v in (width, height, downsampling))
+        if downsampling < 1 or width < downsampling or height < downsampling:
+            raise ValueError(f"render_surface: need downsampling >= 1 and width, height >= downsampling, got "
+                             f"{width}x{height} / {downsampling}")
+        net = self.get_network()
+        level = net.surface_level(level)
+        net._check_trace_args(self.dist_near, self.dist_far, max_steps)
+        w, h = width // downsampling, height // downsampling
+        device = net.device
+        if device.type != "cuda":
+            raise RuntimeError(f"neddf_b200.NeRFRender renders on CUDA devices only (the module is on {device})")
+        hR, hT, hC = _camera_host(camera)
+        n = w * h
+        with torch.no_grad(), torch.cuda.device(device):
+            ray_dir = torch.empty(n, 3, device=device, dtype=torch.float32)
+            ray_orig = torch.empty(n, 3, device=device, dtype=torch.float32)
+            L.check(L.lib().neddf_make_image_rays(width, height, downsampling, 0, n, hR, hT, hC, L.ptr(ray_dir),
+                                                  L.ptr(ray_orig), L.stream_ptr(device)), "make_image_rays")
+            flat = net.trace_surface(ray_dir, ray_orig, self.dist_near, self.dist_far, level, max_steps)
+        return {k: v.reshape(h, w, -1) for k, v in flat.items()}
+
     def render_field_slice(self, slice_t: float = 0.0, render_size: float = 1.1,
                            render_resolution: int = 128) -> Dict[str, np.ndarray]:
         """Field slice visualisation (nerf_render.py:263-336): uint8 BGR images."""
