@@ -213,7 +213,8 @@ int32_t neddf_field_forward(const neddf_field_t* f, const neddf_field_state_t* s
                             void* stream);
 
 /* Same network, with get_sampling_points/cones fused into the prologue: samples are
- * described by rays + edge distances, nothing of size [n,3] touches HBM. */
+ * described by rays + edge distances, nothing of size [n,3] touches HBM.  With d_color and
+ * d_penalty both NULL the tensor-core engines run the distance trunk and heads only. */
 int32_t neddf_field_forward_rays(const neddf_field_t* f, const neddf_field_state_t* st,
                                  const float* d_ray_dir, const float* d_ray_orig,
                                  const float* d_dists, int64_t n_rays, int32_t n_edges,
@@ -263,7 +264,8 @@ int32_t neddf_field_backward_samples(const neddf_field_t* f, const neddf_field_s
 
 /* BaseNeuralRender.integrate_volume_render (neddf/render/base_neural_render.py:117-172) plus
  * the penalty integration of render_rays (nerf_render.py:153-159).
- * in : dists[n_rays,n_edges], density[n_rays,n_edges], color[n_rays,n_edges,3],
+ * in : dists[n_rays,n_edges], density[n_rays,n_edges], color[n_rays,n_edges,3] (NULL, with
+ *      color_out NULL, when only weights / depth / transmittance are wanted),
  *      penalty[n_rays,n_edges] (NULL to skip)
  * out: weight[n_rays,n_edges-1], depth[n_rays], color_out[n_rays,3], transmittance[n_rays],
  *      penalty_out[n_rays] (NULL to skip).  d_status (int32, may be NULL) gets bit0 set if a

@@ -29,7 +29,7 @@ composite_kernel(const float* __restrict__ dists, const float* __restrict__ dens
   for (int64_t ray = warp; ray < n_rays; ray += n_warps) {
     const float* drow = dists + ray * n_edges;
     const float* srow = density + ray * n_edges;
-    const float* crow = color + ray * n_edges * 3;
+    const float* crow = color ? color + ray * n_edges * 3 : nullptr;  // NULL: weights / depth / T only
     const float* prow = penalty ? penalty + ray * n_edges : nullptr;
     float* wrow = weight ? weight + ray * n_int : nullptr;
 
@@ -65,9 +65,11 @@ composite_kernel(const float* __restrict__ dists, const float* __restrict__ dens
         saw_nan |= (w != w);
         if (wrow) wrow[j] = w;
         acc_d += w * dj;
-        acc_r += w * crow[3 * j + 0];
-        acc_g += w * crow[3 * j + 1];
-        acc_b += w * crow[3 * j + 2];
+        if (crow) {
+          acc_r += w * crow[3 * j + 0];
+          acc_g += w * crow[3 * j + 1];
+          acc_b += w * crow[3 * j + 2];
+        }
         if (prow) acc_p += delta * prow[j];
       }
       carry = carry * __shfl_sync(0xffffffffu, incl, 31);
@@ -242,7 +244,8 @@ extern "C" int32_t neddf_composite(const float* d_dists, const float* d_density,
                                    float* d_penalty_out, int32_t* d_status, void* stream) {
   if (n_rays < 0 || n_edges < 1) return fail(NEDDF_E_INVALID, "neddf_composite: bad sizes");
   if (n_rays == 0) return NEDDF_OK;
-  if (!d_dists || !d_density || !d_color) return fail(NEDDF_E_INVALID, "neddf_composite: null input pointer");
+  if (!d_dists || !d_density) return fail(NEDDF_E_INVALID, "neddf_composite: null input pointer");
+  if (d_color_out && !d_color) return fail(NEDDF_E_INVALID, "neddf_composite: color_out without color");
   if (d_penalty_out && !d_penalty) return fail(NEDDF_E_INVALID, "neddf_composite: penalty_out without penalty");
   int64_t blocks = (n_rays + kWarpsPerBlock - 1) / kWarpsPerBlock;
   int64_t cap = (int64_t)sm_count() * 8;  // 8 resident 256-thread CTAs per SM

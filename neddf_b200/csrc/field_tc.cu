@@ -15,7 +15,9 @@
 // d/dy, d/dz), so the value rows are the first 32 rows of every operand.  When only images are
 // wanted (no fields_penalty) the colour trunk needs the value rows alone: a CTA runs the distance
 // trunk of 4 tiles one after the other, parks each tile's value rows in global scratch, and then runs
-// the colour trunk once on the 4 tiles' value rows (row j*32 + s = tile j, sample s), N = 128.
+// the colour trunk once on the 4 tiles' value rows (row j*32 + s = tile j, sample s), N = 128.  A launch that
+// wants neither colour nor penalty nor training state (an image's coarse pass: only its weights, i.e. densities, are
+// used) runs the distance trunk and the distance / aux head alone: no colour inputs, no park, no colour trunk.
 //
 // Orientation.  The MMAs are issued "swapped": A = weights (M = output channels, K-major), B =
 // activations (N = 128 rows = 32 samples x 4, MN-major in shared memory), so a thread's accumulator
@@ -91,6 +93,7 @@ struct TcParams {
   const float* bias;          // [n_hidden][256] plain channel order
   int* status;
   int eval;                   // 1 = images only: colour trunk per group of tiles on value rows, no penalty / colour Jacobian
+  int density_only;           // 1 = no colour, penalty or training output: distance trunk and distance / aux head only
   unsigned char* park;        // kGroup x kParkBytes per CTA (images only)
 };
 
@@ -270,8 +273,10 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
   if (unit < units_total) my_tiles = (units_total - 1 - unit) / n_units + 1;
   auto tile_of = [&](int64_t t) { return PAIR ? 2 * (unit + t * n_units) + rank : unit + t * n_units; };
   // images-only launches take their tiles in groups of kGroup and run the colour trunk once per group (both CTAs
-  // of a pair have the same my_tiles, hence the same groups and the same chunk stream)
-  const int group = P.eval ? kGroup : 1;
+  // of a pair have the same my_tiles, hence the same groups and the same chunk stream).  Density-only launches run no
+  // colour trunk: one tile per group, and the producer streams the distance chunks alone.
+  const int group = P.eval && !P.density_only ? kGroup : 1;
+  const int chunks_end = P.density_only ? P.dist_chunks : P.chunks_per_tile;
 
   if (tid == 0) {
     for (int i = 0; i < kStages; ++i) {
@@ -303,7 +308,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
         const int gn = (int)std::min<int64_t>(group, my_tiles - base);
         for (int i = 0; i < gn; ++i)
           for (int c = 0; c < P.dist_chunks; ++c) push(c);
-        for (int c = P.dist_chunks; c < P.chunks_per_tile; ++c) push(c);
+        for (int c = P.dist_chunks; c < chunks_end; ++c) push(c);
       }
     }
   } else {
@@ -477,8 +482,10 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
           aux[0] += __ldg(p.b_head + 1);
           head_density(ddf, aux, p.d_near, p.aux_grad_scale, p.density_act, head);
           const int kn = p.n_e0 + p.n_d;  // normal: detached, zero Jacobian (neddf.py:243-253)
+          if (!P.density_only) {
 #pragma unroll
-          for (int c = 0; c < 3; ++c) store_sample(aux_hi, aux_lo, kAuxK, hs, kn + c, head.normal[c], 0.f, 0.f, 0.f, bad, rows);
+            for (int c = 0; c < 3; ++c) store_sample(aux_hi, aux_lo, kAuxK, hs, kn + c, head.normal[c], 0.f, 0.f, 0.f, bad, rows);
+          }
           const int64_t n = n0 + hs;
           if (n < n_total) {
             int64_t ray_, on;  // where this sample's outputs go (segment view: [ray, edge] of the full arrays)
@@ -490,7 +497,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
           }
         }
         // colour-trunk inputs E0 | D (| zero pad) into AUX (neddf.py:205-210, 243); the trunk is done with E_s
-        {
+        if (!P.density_only) {
           const int s = tid >> 3, sub = tid & 7;
           write_pos_embedding(p, sc->geo, aux_hi, aux_lo, s, sub, 8, false, bad, rows);
           const int dhalf = 3 * p.embed_dir;
@@ -597,11 +604,12 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
         if (tid == 0) ++ph_sum[kPhTiles];
 #endif
         for (int l = 0; l < p.n_ddf; ++l) layer(l, base + gi, 1);
-        if (P.eval) {  // park this tile's colour-trunk operand until the group's colour pass
+        if (P.eval && !P.density_only) {  // park this tile's colour-trunk operand until the group's colour pass
           park_move<false>(smem, park + gi * kParkBytes, 0, tid);
           TC_PHASE(kPhPark);
         }
       }
+      if (P.density_only) continue;
       if (P.eval) {
         // the group's colour-trunk operand: slot j into row blocks 4j .. 4j + 3 of H and AUX, zeros past its end
         bar_consumers();
@@ -828,7 +836,8 @@ int32_t launch_field_tc(const neddf_field* f, FieldParams& p, int flags, bool pa
   P.bias = S->d_bias;
   P.status = S->d_status;
   P.eval = (flags == NEDDF_OUT_EVAL && p.penalty == nullptr && p.save_pre == nullptr) ? 1 : 0;
-  if (P.eval && !S->d_park) {  // on the first images-only launch: one CTA per SM at most (grids below)
+  P.density_only = (p.color == nullptr && p.penalty == nullptr && p.save_pre == nullptr) ? 1 : 0;
+  if (P.eval && !P.density_only && !S->d_park) {  // on the first images-only launch: one CTA per SM at most (grids below)
     if (cudaMalloc(&S->d_park, (size_t)sm_count() * tc::kGroup * tc::kParkBytes) != cudaSuccess) {
       S->d_park = nullptr;
       return fail(NEDDF_E_CUDA, "tensor-core engine: cudaMalloc of the colour-trunk scratch failed");

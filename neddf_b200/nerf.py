@@ -204,7 +204,7 @@ class NeRF(BaseNeuralField):
         return out
 
     def forward_rays(self, ray_dir: Tensor, ray_orig: Tensor, dists: Tensor, sampling_type: str, ray_radius: float,
-                     need_penalty: bool = True, need_aux: bool = True) -> Dict[str, Tensor]:
+                     need_penalty: bool = True, need_aux: bool = True, need_color: bool = True) -> Dict[str, Tensor]:
         """Same network with the sample geometry fused into the kernel (what NeRFRender calls; the NeRF variant has
         neither penalties nor auxiliary fields, the flags are accepted for interface parity)."""
         ray_dir = L.require_cuda_f32(ray_dir, "ray_dir")

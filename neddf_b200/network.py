@@ -606,10 +606,12 @@ class NeDDF(BaseNeuralField):
         return out
 
     def forward_rays(self, ray_dir: Tensor, ray_orig: Tensor, dists: Tensor, sampling_type: str, ray_radius: float,
-                     need_penalty: bool = True, need_aux: bool = True) -> Dict[str, Tensor]:
+                     need_penalty: bool = True, need_aux: bool = True, need_color: bool = True) -> Dict[str, Tensor]:
         """Same network with the sample geometry fused into the kernel prologue (no [N,3]
         Sampling tensors in HBM).  Used by NeRFRender.  Under autograd (training) it runs the
-        differentiable fp32 path (_FieldTrainFn) and returns density / color / fields_penalty."""
+        differentiable fp32 path (_FieldTrainFn) and returns density / color / fields_penalty.
+        ``need_color=False`` (with ``need_penalty=False``) leaves "color" out: the tensor-core engines then skip
+        the colour trunk, which is what an image's coarse pass wants (only its densities reach the image)."""
         ray_dir = L.require_cuda_f32(ray_dir, "ray_dir")
         ray_orig = L.require_cuda_f32(ray_orig, "ray_orig")
         dists = L.require_cuda_f32(dists, "dists")
@@ -619,10 +621,9 @@ class NeDDF(BaseNeuralField):
             return {"density": d, "color": c, "fields_penalty": pnl}
         B, S = dists.shape
         device = dists.device
-        out = {
-            "density": torch.empty(B, S, device=device, dtype=torch.float32),
-            "color": torch.empty(B, S, 3, device=device, dtype=torch.float32),
-        }
+        out = {"density": torch.empty(B, S, device=device, dtype=torch.float32)}
+        if need_color or need_penalty:
+            out["color"] = torch.empty(B, S, 3, device=device, dtype=torch.float32)
         if need_penalty:
             out["fields_penalty"] = torch.empty(B, S, device=device, dtype=torch.float32)
         if need_aux:
@@ -633,7 +634,7 @@ class NeDDF(BaseNeuralField):
         with self._profiled(device, B * S), torch.cuda.device(device):
             L.check(L.lib().neddf_field_forward_rays(
                 h, C.byref(st), L.ptr(ray_dir), L.ptr(ray_orig), L.ptr(dists), B, S, L.SAMPLING_IDS[sampling_type],
-                float(ray_radius), L.ptr(out.get("distance")), L.ptr(out["density"]), L.ptr(out["color"]),
+                float(ray_radius), L.ptr(out.get("distance")), L.ptr(out["density"]), L.ptr(out.get("color")),
                 L.ptr(out.get("fields_penalty")), L.ptr(out.get("aux_grad")),
                 L.OUT_FULL if need_penalty else L.OUT_EVAL, self._engine_id(), L.stream_ptr(device)),
                 "field_forward_rays")

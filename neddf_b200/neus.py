@@ -230,7 +230,7 @@ class NeuS(BaseNeuralField):
         return out
 
     def forward_rays(self, ray_dir: Tensor, ray_orig: Tensor, dists: Tensor, sampling_type: str, ray_radius: float,
-                     need_penalty: bool = True, need_aux: bool = True, with_normal: bool = False) -> Dict[str, Tensor]:
+                     need_penalty: bool = True, need_aux: bool = True, need_color: bool = True, with_normal: bool = False) -> Dict[str, Tensor]:
         """Same network with the sample geometry fused into the kernel (what NeRFRender calls; this variant has
         neither penalties nor auxiliary fields, the flags are accepted for interface parity)."""
         wants_grad = self._wants_grad()

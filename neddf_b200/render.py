@@ -171,16 +171,21 @@ class BaseNeuralRender(nn.Module):
         return (out, ids) if return_ids else out
 
     # ---- a15 ---------------------------------------------------------------------------
-    def integrate_volume_render(self, dists: Tensor, densities: Tensor, colors: Tensor,
+    def integrate_volume_render(self, dists: Tensor, densities: Tensor, colors: Optional[Tensor],
                                 penalties: Optional[Tensor] = None) -> Dict[str, Tensor]:
         """Alpha compositing (base_neural_render.py:117-172); with ``penalties`` also the
-        per-ray penalty integral of render_rays (nerf_render.py:153-159)."""
+        per-ray penalty integral of render_rays (nerf_render.py:153-159).  ``colors=None`` (no-grad only)
+        composites weight, depth and transmittance alone, with no "color" key."""
         dists = L.require_cuda_f32(dists, "dists")
         densities = L.require_cuda_f32(densities, "densities")
-        colors = L.require_cuda_f32(colors, "colors")
+        if colors is None:
+            if torch.is_grad_enabled() and densities.requires_grad:
+                raise ValueError("integrate_volume_render: colors=None has no backward")
+        else:
+            colors = L.require_cuda_f32(colors, "colors")
         B, E = dists.shape
         device = dists.device
-        if torch.is_grad_enabled() and (densities.requires_grad or colors.requires_grad or
+        if torch.is_grad_enabled() and (densities.requires_grad or (colors is not None and colors.requires_grad) or
                                         (penalties is not None and penalties.requires_grad)):
             if penalties is not None:
                 penalties = L.require_cuda_f32(penalties, "penalties")
@@ -193,9 +198,10 @@ class BaseNeuralRender(nn.Module):
         res = {
             "weight": torch.empty(B, E - 1, device=device, dtype=torch.float32),
             "depth": torch.empty(B, device=device, dtype=torch.float32),
-            "color": torch.empty(B, 3, device=device, dtype=torch.float32),
             "transmittance": torch.empty(B, device=device, dtype=torch.float32),
         }
+        if colors is not None:
+            res["color"] = torch.empty(B, 3, device=device, dtype=torch.float32)
         pen_out = None
         if penalties is not None:
             penalties = L.require_cuda_f32(penalties, "penalties")
@@ -204,7 +210,7 @@ class BaseNeuralRender(nn.Module):
         with torch.cuda.device(device):
             L.check(L.lib().neddf_composite(L.ptr(dists), L.ptr(densities), L.ptr(colors), L.ptr(penalties), B, E,
                                             float(self.max_dist), L.ptr(res["weight"]), L.ptr(res["depth"]),
-                                            L.ptr(res["color"]), L.ptr(res["transmittance"]), L.ptr(pen_out),
+                                            L.ptr(res.get("color")), L.ptr(res["transmittance"]), L.ptr(pen_out),
                                             L.ptr(status), L.stream_ptr(device)), "composite")
         if pen_out is not None:
             res["fields_penalty"] = pen_out
@@ -315,10 +321,12 @@ class NeRFRender(BaseNeuralRender):
 
     # ------------------------------------------------------------------- the hot function --
     def _render_core(self, ray_dir: Tensor, ray_orig: Tensor, u_coarse: Tensor, u_fine: Tensor,
-                     full: bool) -> Dict[str, Tensor]:
+                     full: bool, coarse_color: bool = True) -> Dict[str, Tensor]:
         """render_rays after ray generation (nerf_render.py:130-188).  ``full`` = produce every
         key of the reference dictionary (penalties included); otherwise only what
-        color/depth/transmittance images need."""
+        color/depth/transmittance images need.  ``coarse_color=False`` (images only) evaluates the coarse
+        network for densities alone, since only the coarse weights reach the image, and leaves
+        "color_coarse" out."""
         lib = L.lib()
         B = ray_dir.shape[0]
         device = ray_dir.device
@@ -328,8 +336,8 @@ class NeRFRender(BaseNeuralRender):
         L.check(lib.neddf_coarse_dists(L.ptr(u_coarse), B, Ec, self.dist_near, self.dist_far, L.ptr(dists_c), stream),
                 "coarse_dists")
         vc = self.network_coarse.forward_rays(ray_dir, ray_orig, dists_c, self.sampling_type, self._ray_radius,
-                                              need_penalty=full, need_aux=False)
-        ic = self.integrate_volume_render(dists_c, vc["density"], vc["color"], vc.get("fields_penalty"))
+                                              need_penalty=full, need_aux=False, need_color=full or coarse_color)
+        ic = self.integrate_volume_render(dists_c, vc["density"], vc.get("color"), vc.get("fields_penalty"))
         dists_f = self.sample_pdf(dists_c, ic["weight"], Ef_new, uniform_rands=u_fine)
         if (not full and self.transmittance_eps > 0.0 and not torch.is_grad_enabled()
                 and hasattr(self.network_fine, "forward_rays_segment")):
@@ -442,6 +450,7 @@ class NeRFRender(BaseNeuralRender):
         """Rows [first, first+count) of the row-major pixel list of render_image, as flat
         [count, C] tensors.  This is the unit of work that is sharded across GPUs."""
         target_types = list(target_types)
+        coarse_color = any(k.endswith("_coarse") for k in target_types)  # else the coarse pass runs density-only
         lib = L.lib()
         device = torch.device(device) if device is not None else self.network_fine.device
         if device.type != "cuda":
@@ -462,7 +471,7 @@ class NeRFRender(BaseNeuralRender):
                 else:
                     u = (uniforms[0][b0 - first:b0 - first + n], uniforms[1][b0 - first:b0 - first + n])
                 u_c, u_f = self._uniforms(n, device, u)
-                res = self._render_core(ray_dir, ray_orig, u_c, u_f, full=False)
+                res = self._render_core(ray_dir, ray_orig, u_c, u_f, full=False, coarse_color=coarse_color)
                 for k in target_types:
                     outs[k].append(res[k].reshape(n, -1))
         return {k: (torch.cat(v, 0) if len(v) != 1 else v[0]) for k, v in outs.items()}
