@@ -317,12 +317,12 @@ int32_t neddf_tc_selftest(const float* d_a, const float* d_b, int32_t m, int32_t
 
 /* ------------------------------------------------------------------------------------------------
  * NeRF field variant (SURVEY 8(f) item 3; neddf/network/nerf.py).  Forward only, fp32 CUDA-core kernel
- * (csrc/nerf_simt.cu): the same renderer entry points (coarse_dists, composite, sample_pdf) serve it.
+ * (csrc/nerf_simt.cu + csrc/nerf_kernel.cuh): the same renderer entry points (coarse_dists, composite, sample_pdf) serve it.
  * ------------------------------------------------------------------------------------------------ */
 typedef struct neddf_nerf_config {
   int32_t embed_pos_rank;          /* nerf.py:36 (6 * rank <= 64) */
   int32_t embed_dir_rank;          /* nerf.py:37 (6 * rank <= 32) */
-  int32_t layer_count;             /* nerf.py:38, 2..12 */
+  int32_t layer_count;             /* nerf.py:38, 2..13 (training backward: 2..12) */
   int32_t layer_width;             /* nerf.py:39, must be 256 */
   int32_t activation_type;         /* NEDDF_ACT_* (nerf.py:40) */
   int32_t density_activation_type; /* NEDDF_ACT_* (nerf.py:41) */

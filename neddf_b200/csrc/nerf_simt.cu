@@ -1,24 +1,9 @@
 // NeRF field variant (SURVEY 8(f) item 3): the reference's vanilla NeRF MLP as one persistent CUDA-core kernel.
-//
-// Reference: NeRF.forward (neddf/network/nerf.py:107-165): position embedding with low-pass x sample-size weights
-// (:133-141), `layer_count` hidden layers with skip concat [h | E] AFTER the layers named in `skips` (:144-148),
-// density head + density activation (:149), colour branch Linear(width + dir embedding -> width/2), ReLU,
-// Linear(-> 3) (:96-103, :151-153).  Sample geometry optionally fused like the NeDDF kernels
-// (Ray.get_sampling_points / get_sampling_cones, neddf/ray/ray.py:88-194).
-//
-// First CUDA statement of this variant: every multiply-add is an fp32 FMA (parity class of the fp32 NeDDF engine);
-// it does not use the tensor cores yet.  Forward only - the NeRF variant trains through the reference.
-//
-// Work decomposition
-//   CTA (256 threads) = tile of 64 samples, grid = #SMs, persistent over tiles.
-//   Activations live K-major in shared memory: E[k][s] (position embedding), D[k][s] (direction embedding),
-//   H[c][s] (hidden features, rewritten in place layer after layer).  A layer reads one or two row segments
-//   (H then E for the layer behind a skip, H then D for the colour branch), so the concats move no data.
-//   Thread (cg = tid % 16, sg = tid / 16) owns samples 4 sg .. 4 sg + 3 and the 16 output channels
-//   {4 cg + 64 i + j}: per input row one float4 of activations, four conflict-free float4 of weights, 64 FMAs.
-//   Weights: packed once as [in rows, padded to 16][256 outputs, padded] fp32, streamed through a
-//   double-buffered 16-row shared-memory chunk with cp.async; the model (2.4 MB) stays in L2.
-#include "field_math.cuh"
+// The tile program (layer table, prologue, activations, GEMM loop) lives in nerf_kernel.cuh, which the training backward
+// (nerf_train_kernel.cuh) recomputes the forward with and which is also compiled by g++ into a host emulation for the
+// CPU tests; this file supplies the kernel wrapper, the weight packer of both NeRF handles and the C ABI
+// (neddf_nerf_*).  Forward only, fp32 FMA (parity class of the fp32 NeDDF engine).
+#include "nerf_kernel.cuh"
 
 #include <algorithm>
 #include <cstring>
@@ -26,243 +11,12 @@
 namespace neddf {
 namespace nerf {
 
-constexpr int kT = 64;         // samples per tile
-constexpr int kW = 256;        // layer width (fixed)
-constexpr int kChunk = 16;     // weight rows per shared-memory chunk
-constexpr int kMaxE = 64;      // rows reserved for the position embedding (6 * rank <= 64)
-constexpr int kMaxD = 32;      // direction embedding (6 * rank <= 32)
-constexpr int kMaxLayers = 14; // hidden layers + colour layer
-constexpr int kThreads = 256;
-
-enum Seg { kSegNone = 0, kSegE = 1, kSegH = 2, kSegD = 3 };
-
-struct Layer {
-  int w_off;     // float offset of the packed [k_pad][256] block
-  int b_off;     // float offset of the [256] bias block
-  int k_pad;     // input rows padded to a multiple of kChunk
-  int seg_a, n_a;  // first input segment and its rows
-  int seg_b, n_b;  // second one (kSegNone: none)
-  int act;       // NEDDF_ACT_*
-};
-
-struct Params {
-  // network
-  int n_layers;  // hidden layers; layer n_layers is the colour branch's first layer
-  Layer layer[kMaxLayers];
-  const float* w;  // packed weights + biases
-  int embed_pos, embed_dir, n_e, n_d;
-  int density_act;
-  int w_density_off, w_col2_off;  // [256] + bias ; [3][128] + 3 biases
-  float lowpass[16];
-  // inputs: explicit samples or rays + edges
-  int64_t n;
-  const float *pos, *dir, *var;
-  const float *ray_dir, *ray_orig, *dists;
-  int n_edges, sampling_type;
-  float ray_radius;
-  // outputs
-  float* density;
-  float* color;
-};
-
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-__device__ __forceinline__ float act_value(int act, float x) {
-  float y, d;
-  if (act == NEDDF_ACT_TANHEXP) hidden_act<NEDDF_ACT_TANHEXP>(x, y, d);
-  else if (act == NEDDF_ACT_RELU) hidden_act<NEDDF_ACT_RELU>(x, y, d);
-  else hidden_act<NEDDF_ACT_LEAKYRELU>(x, y, d);
-  return y;
-}
-
 __global__ void __launch_bounds__(kThreads, 1) nerf_forward_kernel(const __grid_constant__ Params P) {
   extern __shared__ __align__(16) float smem[];
-  float* E = smem;                       // [kMaxE][kT]
-  float* D = E + kMaxE * kT;             // [kMaxD][kT]
-  float* H = D + kMaxD * kT;             // [kW][kT]
-  float* Wc = H + kW * kT;               // [2][kChunk][kW]
-  __shared__ float geo[kT][9];           // pos, dir, var
-
-  const int tid = threadIdx.x;
-  const int cg = tid & 15, sg = tid >> 4;
-  const int64_t n_tiles = (P.n + kT - 1) / kT;
-
-  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const int64_t n0 = tile * kT;
-    // ---- geometry of the tile's samples (one thread per sample) --------------------------------------
-    if (tid < kT) {
-      float pos[3] = {0.f, 0.f, 0.f}, dir[3] = {0.f, 0.f, 1.f}, var[3] = {0.f, 0.f, 0.f};
-      const int64_t n = n0 + tid;
-      if (n < P.n) {
-        if (P.dists) {
-          const int64_t b = n / P.n_edges;
-          const int j = (int)(n - b * P.n_edges);
-          const float* row = P.dists + b * P.n_edges;
-          float o[3];
-#pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            o[i] = P.ray_orig[3 * b + i];
-            dir[i] = P.ray_dir[3 * b + i];
-          }
-          sample_geometry(P.sampling_type, P.ray_radius, o, dir, row[j], far_edge(row, j, P.n_edges), pos, var);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            pos[i] = P.pos[3 * n + i];
-            dir[i] = P.dir[3 * n + i];
-            var[i] = P.var[3 * n + i];
-          }
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        geo[tid][i] = pos[i];
-        geo[tid][3 + i] = dir[i];
-        geo[tid][6 + i] = var[i];
-      }
-    }
-    __syncthreads();
-    // ---- embeddings (nerf.py:133-142): four threads per sample --------------------------------------
-    {
-      const int s = tid >> 2, sub = tid & 3;
-      const int half3 = 3 * P.embed_pos;
-      for (int idx = sub; idx < half3; idx += 4) {
-        const int e = idx / 3, d = idx - 3 * e;
-        const PeEntry q = pe_entry(e, geo[s][d], geo[s][6 + d], P.lowpass[e]);
-        E[idx * kT + s] = q.scale_0 * q.s;
-        E[(half3 + idx) * kT + s] = q.scale_0 * q.c;
-      }
-      const int dhalf = 3 * P.embed_dir;
-      for (int idx = sub; idx < dhalf; idx += 4) {
-        const int e = idx / 3, d = idx - 3 * e;
-        float sn, cs;
-        sincosf((float)(1u << e) * geo[s][3 + d], &sn, &cs);
-        D[idx * kT + s] = sn;
-        D[(dhalf + idx) * kT + s] = cs;
-      }
-    }
-    __syncthreads();
-
-    // ---- layers ----------------------------------------------------------------------------------
-    for (int l = 0; l <= P.n_layers; ++l) {
-      if (l == P.n_layers) {
-        // density head on the trunk's features, before the colour branch overwrites H (nerf.py:149)
-        if (tid < kT) {
-          const float* wd = P.w + P.w_density_off;
-          float acc = wd[kW];
-          for (int c = 0; c < kW; ++c) acc = fmaf(__ldg(wd + c), H[c * kT + tid], acc);
-          const int64_t n = n0 + tid;
-          if (n < P.n) P.density[n] = density_act(P.density_act, acc);
-        }
-        // (no barrier needed: the layer below starts by reading H and only writes it after its own barriers)
-      }
-      const Layer& L = P.layer[l];
-      auto seg_ptr = [&](int seg) -> const float* { return seg == kSegE ? E : (seg == kSegD ? D : H); };
-      const float* A = seg_ptr(L.seg_a);
-      const float* B = seg_ptr(L.seg_b);
-      const float* wl = P.w + L.w_off;
-      const int n_chunks = L.k_pad / kChunk;
-      float acc[4][4][4];  // [i][j][sample]
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-#pragma unroll
-          for (int s = 0; s < 4; ++s) acc[i][j][s] = 0.f;
-      auto load_chunk = [&](int buf, int c) {
-        const float4* src = reinterpret_cast<const float4*>(wl + (size_t)c * kChunk * kW);
-        float4* dst = reinterpret_cast<float4*>(Wc + buf * kChunk * kW);
-#pragma unroll
-        for (int u = 0; u < (kChunk * kW / 4) / kThreads; ++u) cp_async16(dst + tid + u * kThreads, src + tid + u * kThreads);
-        cp_commit();
-      };
-      load_chunk(0, 0);
-      for (int c = 0; c < n_chunks; ++c) {
-        if (c + 1 < n_chunks) {
-          load_chunk((c + 1) & 1, c + 1);
-          cp_wait<1>();
-        } else {
-          cp_wait<0>();
-        }
-        __syncthreads();
-        const float* wc = Wc + (c & 1) * kChunk * kW;
-#pragma unroll 4
-        for (int kk = 0; kk < kChunk; ++kk) {
-          const int k = c * kChunk + kk;
-          // rows beyond the layer's inputs carry zero weights; they read row 0 of the first segment
-          const float* rowp = (k < L.n_a) ? A + k * kT : ((k < L.n_a + L.n_b) ? B + (k - L.n_a) * kT : A);
-          const float4 a = *reinterpret_cast<const float4*>(rowp + 4 * sg);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float4 w4 = *reinterpret_cast<const float4*>(wc + kk * kW + 4 * cg + 64 * i);
-            const float wv[4] = {w4.x, w4.y, w4.z, w4.w};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              acc[i][j][0] = fmaf(wv[j], a.x, acc[i][j][0]);
-              acc[i][j][1] = fmaf(wv[j], a.y, acc[i][j][1]);
-              acc[i][j][2] = fmaf(wv[j], a.z, acc[i][j][2]);
-              acc[i][j][3] = fmaf(wv[j], a.w, acc[i][j][3]);
-            }
-          }
-        }
-        __syncthreads();  // chunk buffer free; after the last chunk: every thread is done reading H
-      }
-      // bias + activation, in place
-      const float* bl = P.w + L.b_off;
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int ch = 4 * cg + 64 * i + j;
-          const float b = __ldg(bl + ch);
-          float4 o;
-          o.x = act_value(L.act, acc[i][j][0] + b);
-          o.y = act_value(L.act, acc[i][j][1] + b);
-          o.z = act_value(L.act, acc[i][j][2] + b);
-          o.w = act_value(L.act, acc[i][j][3] + b);
-          *reinterpret_cast<float4*>(H + ch * kT + 4 * sg) = o;
-        }
-      __syncthreads();
-    }
-    // ---- colour output (nerf.py:101-102): 3 x (width / 2) ------------------------------------------
-    if (tid < kT) {
-      const float* wc2 = P.w + P.w_col2_off;
-      const int64_t n = n0 + tid;
-      float o[3];
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        float acc = wc2[3 * (kW / 2) + c];
-        for (int k = 0; k < kW / 2; ++k) acc = fmaf(__ldg(wc2 + c * (kW / 2) + k), H[k * kT + tid], acc);
-        o[c] = acc;
-      }
-      if (n < P.n) {
-        P.color[3 * n + 0] = o[0];
-        P.color[3 * n + 1] = o[1];
-        P.color[3 * n + 2] = o[2];
-      }
-    }
-    __syncthreads();  // H, E, D, geo are rewritten by the next tile
-  }
+  simt::CudaCtx cx{(int)threadIdx.x, (int)blockIdx.x, (int)gridDim.x};
+  tile_program(cx, P, smem);
 }
 
-constexpr size_t kSmemBytes = (size_t)(kMaxE * kT + kMaxD * kT + kW * kT + 2 * kChunk * kW) * sizeof(float);
-
-// torch Linear weights [out][in] -> [in padded][256 padded], biases -> [256]
-__global__ void nerf_pack_kernel(const float* __restrict__ w, const float* __restrict__ b, int n_in, int n_out, int k_pad,
-                                 float* __restrict__ dst_w, float* __restrict__ dst_b) {
-  const int total = k_pad * kW;
-  for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
-    const int k = idx / kW, c = idx - k * kW;
-    dst_w[idx] = (k < n_in && c < n_out) ? w[(size_t)c * n_in + k] : 0.f;
-  }
-  if (blockIdx.x == 0)
-    for (int c = threadIdx.x; c < kW; c += blockDim.x) dst_b[c] = c < n_out ? b[c] : 0.f;
-}
 // small heads: density [256] + bias, colour [3][128] + 3 biases, as stored by torch
 __global__ void nerf_pack_heads_kernel(const float* __restrict__ wd, const float* __restrict__ bd, const float* __restrict__ wc,
                                        const float* __restrict__ bc, float* __restrict__ dst_d, float* __restrict__ dst_c) {
@@ -270,6 +24,22 @@ __global__ void nerf_pack_heads_kernel(const float* __restrict__ wd, const float
   if (threadIdx.x == 0) dst_d[kW] = bd[0];
   for (int i = threadIdx.x; i < 3 * (kW / 2); i += blockDim.x) dst_c[i] = wc[i];
   if (threadIdx.x < 3) dst_c[3 * (kW / 2) + threadIdx.x] = bc[threadIdx.x];
+}
+
+int32_t pack_weights(const Params& P, const int* shape_in, const int* shape_out, const float* const* d_w, const float* const* d_b,
+                     float* dst, cudaStream_t s) {
+  // hidden layers 0..L-1 are tensors 0..L-1; the colour branch's first layer (kernel layer L) is tensor L + 1
+  const int L = P.n_layers;
+  for (int l = 0; l <= L; ++l) {
+    const int t = (l < L) ? l : L + 1;
+    const Layer& ly = P.layer[l];
+    simt::pack_linear_kernel<<<64, 256, 0, s>>>(d_w[t], d_b[t], shape_in[t], shape_out[t], ly.k_pad, ly.kt_pad, 0, dst + ly.w_off,
+                                                dst + ly.b_off, dst + ly.wt_off);
+    NEDDF_LAUNCH_CHECK();
+  }
+  nerf_pack_heads_kernel<<<1, 256, 0, s>>>(d_w[L], d_b[L], d_w[L + 2], d_b[L + 2], dst + P.w_density_off, dst + P.w_col2_off);
+  NEDDF_LAUNCH_CHECK();
+  return NEDDF_OK;
 }
 
 }  // namespace nerf
@@ -282,7 +52,6 @@ using namespace neddf;
 
 struct neddf_nerf {
   neddf_nerf_config_t cfg;
-  int n_hidden = 0;
   int shape_in[nerf::kMaxLayers + 3];
   int shape_out[nerf::kMaxLayers + 3];
   nerf::Params proto;  // structure filled at creation
@@ -291,31 +60,10 @@ struct neddf_nerf {
   bool packed = false;
 };
 
-static bool nerf_is_skip(const neddf_nerf_config_t* c, int lid) {
-  for (int i = 0; i < c->n_skips; ++i)
-    if (c->skips[i] == lid) return true;
-  return false;
-}
-
-// layers.0 .. layers.{L-1}, outL_density, outL_color.0, outL_color.2 (nerf.py:86-103)
-static int nerf_shapes(const neddf_nerf_config_t* c, int* sin, int* sout) {
-  const int in_pos = 6 * c->embed_pos_rank, in_dir = 6 * c->embed_dir_rank, W = c->layer_width;
-  int n = 0;
-  sin[n] = in_pos; sout[n++] = W;
-  for (int lid = 0; lid < c->layer_count - 1; ++lid) {
-    sin[n] = W + (nerf_is_skip(c, lid) ? in_pos : 0);
-    sout[n++] = W;
-  }
-  sin[n] = W; sout[n++] = 1;
-  sin[n] = W + in_dir; sout[n++] = W / 2;
-  sin[n] = W / 2; sout[n++] = 3;
-  return n;
-}
-
 extern "C" int32_t neddf_nerf_layer_shapes(const neddf_nerf_config_t* cfg, int32_t* shapes_out, int32_t max_layers) {
   if (!cfg || cfg->layer_count < 2 || cfg->layer_count > nerf::kMaxLayers - 1) return fail(NEDDF_E_INVALID, "neddf_nerf_layer_shapes: bad config");
   int sin[nerf::kMaxLayers + 3], sout[nerf::kMaxLayers + 3];
-  const int n = nerf_shapes(cfg, sin, sout);
+  const int n = nerf::layer_shapes(cfg, sin, sout);
   if (shapes_out) {
     if (max_layers < n) return fail(NEDDF_E_INVALID, "neddf_nerf_layer_shapes: buffer too small");
     for (int i = 0; i < n; ++i) {
@@ -328,44 +76,14 @@ extern "C" int32_t neddf_nerf_layer_shapes(const neddf_nerf_config_t* cfg, int32
 
 extern "C" int32_t neddf_nerf_create(const neddf_nerf_config_t* cfg, neddf_nerf_t** out) {
   if (!cfg || !out) return fail(NEDDF_E_INVALID, "neddf_nerf_create: null argument");
-  if (cfg->layer_width != nerf::kW) return fail(NEDDF_E_UNSUPPORTED, "neddf_nerf_create: layer_width must be 256");
-  if (cfg->layer_count < 2 || cfg->layer_count > nerf::kMaxLayers - 1) return fail(NEDDF_E_UNSUPPORTED, "neddf_nerf_create: layer_count must be 2..12");
-  if (cfg->embed_pos_rank < 1 || 6 * cfg->embed_pos_rank > nerf::kMaxE || cfg->embed_pos_rank > 16 || cfg->embed_dir_rank < 1 ||
-      6 * cfg->embed_dir_rank > nerf::kMaxD)
-    return fail(NEDDF_E_UNSUPPORTED, "neddf_nerf_create: embedding ranks must satisfy 6 pos <= 64, 6 dir <= 32");
-  if (cfg->n_skips < 0 || cfg->n_skips > 8) return fail(NEDDF_E_INVALID, "neddf_nerf_create: bad skips");
-  for (int a : {cfg->activation_type, cfg->density_activation_type})
-    if (a != NEDDF_ACT_TANHEXP && a != NEDDF_ACT_RELU && a != NEDDF_ACT_LEAKYRELU) return fail(NEDDF_E_INVALID, "neddf_nerf_create: bad activation");
-  if (nerf_is_skip(cfg, cfg->layer_count - 1))
-    return fail(NEDDF_E_UNSUPPORTED, "neddf_nerf_create: a skip after the last hidden layer widens the heads (not covered)");
+  int32_t code;
+  if (const char* why = nerf::unsupported(cfg, code)) return fail(code, std::string("neddf_nerf_create: ") + why);
   neddf_nerf* h = new neddf_nerf();
   h->cfg = *cfg;
-  h->n_hidden = cfg->layer_count;
-  nerf_shapes(cfg, h->shape_in, h->shape_out);
-  nerf::Params& P = h->proto;
-  std::memset(&P, 0, sizeof(P));
-  P.n_layers = cfg->layer_count;
-  P.embed_pos = cfg->embed_pos_rank;
-  P.embed_dir = cfg->embed_dir_rank;
-  P.n_e = 6 * cfg->embed_pos_rank;
-  P.n_d = 6 * cfg->embed_dir_rank;
-  P.density_act = cfg->density_activation_type;
-  size_t off = 0;
-  auto pad16 = [](int k) { return (k + nerf::kChunk - 1) / nerf::kChunk * nerf::kChunk; };
-  for (int l = 0; l <= cfg->layer_count; ++l) {
-    nerf::Layer& L = P.layer[l];
-    if (l == 0) { L.seg_a = nerf::kSegE; L.n_a = P.n_e; L.seg_b = nerf::kSegNone; L.n_b = 0; }
-    else if (l < cfg->layer_count) { L.seg_a = nerf::kSegH; L.n_a = nerf::kW; L.seg_b = nerf_is_skip(cfg, l - 1) ? nerf::kSegE : nerf::kSegNone; L.n_b = L.seg_b ? P.n_e : 0; }
-    else { L.seg_a = nerf::kSegH; L.n_a = nerf::kW; L.seg_b = nerf::kSegD; L.n_b = P.n_d; }
-    L.act = (l < cfg->layer_count) ? cfg->activation_type : NEDDF_ACT_RELU;  // outL_color's nn.ReLU (nerf.py:100)
-    L.k_pad = pad16(L.n_a + L.n_b);
-    L.w_off = (int)off; off += (size_t)L.k_pad * nerf::kW;
-    L.b_off = (int)off; off += nerf::kW;
-  }
-  P.w_density_off = (int)off; off += nerf::kW + 4;
-  P.w_col2_off = (int)off; off += 3 * (nerf::kW / 2) + 4;
-  h->w_floats = off;
-  if (cudaMalloc(&h->d_w, off * sizeof(float)) != cudaSuccess) {
+  nerf::layer_shapes(cfg, h->shape_in, h->shape_out);
+  std::memset(&h->proto, 0, sizeof(h->proto));
+  h->w_floats = nerf::build_program(cfg, h->proto, /*transposed=*/false);
+  if (cudaMalloc(&h->d_w, h->w_floats * sizeof(float)) != cudaSuccess) {
     delete h;
     return fail(NEDDF_E_CUDA, "neddf_nerf_create: cudaMalloc failed");
   }
@@ -384,17 +102,7 @@ extern "C" int32_t neddf_nerf_set_weights(neddf_nerf_t* h, const float* const* d
   if (!h || !d_w || !d_b) return fail(NEDDF_E_INVALID, "neddf_nerf_set_weights: null argument");
   const int L = h->cfg.layer_count;
   if (n_layers != L + 3) return fail(NEDDF_E_INVALID, "neddf_nerf_set_weights: expected layer_count + 3 layers");
-  cudaStream_t s = (cudaStream_t)stream;
-  // hidden layers 0..L-1 are tensors 0..L-1; the colour branch's first layer (kernel layer L) is tensor L + 1
-  for (int l = 0; l <= L; ++l) {
-    const int t = (l < L) ? l : L + 1;
-    const nerf::Layer& ly = h->proto.layer[l];
-    nerf::nerf_pack_kernel<<<64, 256, 0, s>>>(d_w[t], d_b[t], h->shape_in[t], h->shape_out[t], ly.k_pad, h->d_w + ly.w_off, h->d_w + ly.b_off);
-    NEDDF_LAUNCH_CHECK();
-  }
-  nerf::nerf_pack_heads_kernel<<<1, 256, 0, s>>>(d_w[L], d_b[L], d_w[L + 2], d_b[L + 2], h->d_w + h->proto.w_density_off,
-                                                 h->d_w + h->proto.w_col2_off);
-  NEDDF_LAUNCH_CHECK();
+  if (int32_t rc = nerf::pack_weights(h->proto, h->shape_in, h->shape_out, d_w, d_b, h->d_w, (cudaStream_t)stream)) return rc;
   h->packed = true;
   return NEDDF_OK;
 }

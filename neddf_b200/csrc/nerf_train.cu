@@ -1,5 +1,5 @@
-// NeRF field variant, training backward (SURVEY 8(f) item 3): CUDA thread context, weight packing and C ABI around
-// the tile program of nerf_train_kernel.cuh (which is also compiled by g++ into a host emulation for the CPU tests).
+// NeRF field variant, training backward (SURVEY 8(f) item 3): kernel wrapper and C ABI around the tile program of
+// nerf_train_kernel.cuh (which is also compiled by g++ into a host emulation for the CPU tests).
 // One launch recomputes the forward per 64-sample tile and walks back through the network; it leaves the operands of
 // the weight-gradient GEMMs (layer inputs X, pre-activation gradients G) in global memory for neddf_wgrad.
 #include "nerf_train_kernel.cuh"
@@ -10,39 +10,10 @@
 namespace neddf {
 namespace nerft {
 
-struct CudaCtx {
-  int tid, block, nblocks;
-  __device__ __forceinline__ void sync() { __syncthreads(); }
-  __device__ __forceinline__ void cp16(void* smem, const void* gmem) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
-  }
-  __device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-  __device__ __forceinline__ void cp_wait_1() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
-  __device__ __forceinline__ void cp_wait_0() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
-};
-
 __global__ void __launch_bounds__(kThreads, 1) nerf_train_kernel(const __grid_constant__ Params P) {
   extern __shared__ __align__(16) float smem[];
-  CudaCtx cx{(int)threadIdx.x, (int)blockIdx.x, (int)gridDim.x};
+  simt::CudaCtx cx{(int)threadIdx.x, (int)blockIdx.x, (int)gridDim.x};
   tile_program(cx, P, smem);
-}
-
-// forward pack [k_pad][256] + bias [256] + transposed pack [kt_pad][256] of one torch nn.Linear ([out][in], [out])
-__global__ void nerf_train_pack_kernel(const float* __restrict__ w, const float* __restrict__ b, int n_in, int n_out, int k_pad,
-                                       int kt_pad, float* __restrict__ dst_w, float* __restrict__ dst_b, float* __restrict__ dst_wt) {
-  const int stride = gridDim.x * blockDim.x, t0 = blockIdx.x * blockDim.x + threadIdx.x;
-  for (int idx = t0; idx < k_pad * kW; idx += stride) dst_w[idx] = pack_fwd(w, n_in, n_out, idx / kW, idx % kW);
-  for (int idx = t0; idx < kt_pad * kW; idx += stride) dst_wt[idx] = pack_bwd(w, n_in, n_out, idx / kW, idx % kW);
-  if (blockIdx.x == 0)
-    for (int c = threadIdx.x; c < kW; c += blockDim.x) dst_b[c] = c < n_out ? b[c] : 0.f;
-}
-// density [256] + bias, colour output [3][128] + 3 biases, as stored by torch
-__global__ void nerf_train_pack_heads_kernel(const float* __restrict__ wd, const float* __restrict__ bd, const float* __restrict__ wc,
-                                             const float* __restrict__ bc, float* __restrict__ dst_d, float* __restrict__ dst_c) {
-  for (int i = threadIdx.x; i < kW; i += blockDim.x) dst_d[i] = wd[i];
-  if (threadIdx.x == 0) dst_d[kW] = bd[0];
-  for (int i = threadIdx.x; i < 3 * (kW / 2); i += blockDim.x) dst_c[i] = wc[i];
-  if (threadIdx.x < 3) dst_c[3 * (kW / 2) + threadIdx.x] = bc[threadIdx.x];
 }
 
 }  // namespace nerft
@@ -53,8 +24,8 @@ using namespace neddf;
 struct neddf_nerf_train {
   neddf_nerf_config_t cfg;
   int n_layers = 0;
-  int shape_in[nerft::kMaxLayers + 3];
-  int shape_out[nerft::kMaxLayers + 3];
+  int shape_in[nerf::kMaxLayers + 3];
+  int shape_out[nerf::kMaxLayers + 3];
   nerft::Params proto;
   float* d_w = nullptr;
   size_t w_floats = 0;
@@ -66,7 +37,7 @@ extern "C" int32_t neddf_nerf_train_create(const neddf_nerf_config_t* cfg, neddf
   if (const char* why = nerft::unsupported(cfg)) return fail(NEDDF_E_UNSUPPORTED, std::string("neddf_nerf_train_create: ") + why);
   neddf_nerf_train* h = new neddf_nerf_train();
   h->cfg = *cfg;
-  h->n_layers = nerft::layer_shapes(cfg, h->shape_in, h->shape_out);
+  h->n_layers = nerf::layer_shapes(cfg, h->shape_in, h->shape_out);
   std::memset(&h->proto, 0, sizeof(h->proto));
   h->w_floats = nerft::build_program(cfg, h->proto);
   if (cudaMalloc(&h->d_w, h->w_floats * sizeof(float)) != cudaSuccess) {
@@ -88,18 +59,7 @@ extern "C" int32_t neddf_nerf_train_set_weights(neddf_nerf_train_t* h, const flo
   if (!h || !d_w || !d_b) return fail(NEDDF_E_INVALID, "neddf_nerf_train_set_weights: null argument");
   const int L = h->cfg.layer_count;
   if (n_layers != L + 3) return fail(NEDDF_E_INVALID, "neddf_nerf_train_set_weights: expected layer_count + 3 layers");
-  cudaStream_t s = (cudaStream_t)stream;
-  // hidden layers 0..L-1 are tensors 0..L-1; the colour branch's first layer (kernel layer L) is tensor L + 1
-  for (int l = 0; l <= L; ++l) {
-    const int t = (l < L) ? l : L + 1;
-    const nerft::Layer& ly = h->proto.layer[l];
-    nerft::nerf_train_pack_kernel<<<64, 256, 0, s>>>(d_w[t], d_b[t], h->shape_in[t], h->shape_out[t], ly.k_pad, ly.kt_pad,
-                                                     h->d_w + ly.w_off, h->d_w + ly.b_off, h->d_w + ly.wt_off);
-    NEDDF_LAUNCH_CHECK();
-  }
-  nerft::nerf_train_pack_heads_kernel<<<1, 256, 0, s>>>(d_w[L], d_b[L], d_w[L + 2], d_b[L + 2], h->d_w + h->proto.w_density_off,
-                                                        h->d_w + h->proto.w_col2_off);
-  NEDDF_LAUNCH_CHECK();
+  if (int32_t rc = nerf::pack_weights(h->proto, h->shape_in, h->shape_out, d_w, d_b, h->d_w, (cudaStream_t)stream)) return rc;
   h->packed = true;
   return NEDDF_OK;
 }

@@ -11,7 +11,7 @@
 // (value, d/dx, d/dy, d/dz; the layout of the NeDDF kernels), G = f'(x) (J W) - the same number as the reference's
 // reverse-mode gradient up to rounding (oracle.neus_forward_jac against oracle.neus_forward, tests/test_neus_oracle.py).
 //
-// Work decomposition (the fp32 CUDA-core skeleton of csrc/nerf_simt.cu)
+// Work decomposition (the fp32 CUDA-core skeleton of simt_tile.cuh)
 //   CTA (256 threads) = tile of 64 samples, persistent over tiles.  Activations K-major in shared memory
 //   (row = channel, 64 columns).  SDF trunk: four passes over sub-tiles of 16 samples, column = 4 sample + row type;
 //   the last SDF layer parks its value rows in F (column = sample) and the normal in the colour input head X.
@@ -20,12 +20,12 @@
 //   sg; colour trunk: four samples) and the 16 output channels {4 cg + 64 i + j}.
 //   Weights: [in rows padded to 16][256] fp32, streamed through a double-buffered 16-row chunk (cp.async).
 //
-// This header is compiled twice: by nvcc into the kernel (Ctx = the CUDA thread) and by g++ into
+// This header is compiled twice: by nvcc into the kernel (Ctx = simt::CudaCtx) and by g++ into
 // tests/emul/libneus_emul.so (Ctx = one of 256 OS threads per CTA, a barrier for __syncthreads) so that the very
-// same index arithmetic is checked against the goldens in the build container, which has no GPU.
+// same index arithmetic is checked against the goldens on a machine without a GPU.
 #pragma once
 
-#include "common.cuh"
+#include "simt_tile.cuh"
 
 #ifdef __CUDACC__
 #define NEUS_LDG(p) __ldg(p)
@@ -36,15 +36,16 @@
 namespace neddf {
 namespace neus {
 
-constexpr int kT = 64;       // samples per tile
+using simt::kChunk;
+using simt::kT;
+using simt::kThreads;
+using simt::kW;
+using simt::pack_entry;
 constexpr int kSub = 16;     // samples per SDF sub-tile (4 columns each)
-constexpr int kW = 256;      // layer width (fixed)
-constexpr int kChunk = 16;   // weight rows per shared-memory chunk
 constexpr int kMaxE = 64;    // rows reserved for the position embedding (6 * rank <= 64)
 constexpr int kMaxX = 32;    // colour input head [pos 3 | dir embedding 6 * rank | normal 3] (<= 32 rows)
 constexpr int kMaxSdf = 12;  // SDF layers
 constexpr int kMaxCol = 12;  // colour layers of width 256 (the 3-channel output layer is a per-sample head)
-constexpr int kThreads = 256;
 
 enum Seg { kSegNone = 0, kSegE = 1, kSegH = 2, kSegX = 3, kSegF = 4 };
 
@@ -120,62 +121,12 @@ __device__ __forceinline__ const float* seg_ptr(const float* smem, int seg) {
   return smem + (seg == kSegE ? kOffE : (seg == kSegX ? kOffX : (seg == kSegF ? kOffF : kOffH)));
 }
 
-// acc[i][j][col] = sum_k W[k][4 cg + 64 i + j] * act[k][4 sg + col] over the layer's input rows.
-// Entry: every thread has passed a barrier after the last write to the input segments and after the last read of
-// the weight chunk buffers.  Exit: every thread has finished reading the input segments (trailing barrier).
+// the layer's GEMM (simt::gemm, with its entry / exit barrier contract) over its input segments
 template <class Ctx>
 __device__ __forceinline__ void layer_gemm(Ctx& cx, const Params& P, const Layer& L, float* smem, float (&acc)[4][4][4]) {
-  const int tid = cx.tid;
-  const int cg = tid & 15, sg = tid >> 4;
   const float* A = seg_ptr(smem, L.seg_a);
   const float* B = seg_ptr(smem, L.seg_b);
-  const float* wl = P.w + L.w_off;
-  float* Wc = smem + kOffW;
-  const int n_chunks = L.k_pad / kChunk;
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-#pragma unroll
-      for (int s = 0; s < 4; ++s) acc[i][j][s] = 0.f;
-  auto load_chunk = [&](int buf, int c) {
-    const float* src = wl + (size_t)c * kChunk * kW;
-    float* dst = Wc + buf * kChunk * kW;
-#pragma unroll
-    for (int u = 0; u < (kChunk * kW / 4) / kThreads; ++u) cx.cp16(dst + 4 * (tid + u * kThreads), src + 4 * (tid + u * kThreads));
-    cx.cp_commit();
-  };
-  load_chunk(0, 0);
-  for (int c = 0; c < n_chunks; ++c) {
-    if (c + 1 < n_chunks) {
-      load_chunk((c + 1) & 1, c + 1);
-      cx.cp_wait_1();
-    } else {
-      cx.cp_wait_0();
-    }
-    cx.sync();
-    const float* wc = Wc + (c & 1) * kChunk * kW;
-#pragma unroll 4
-    for (int kk = 0; kk < kChunk; ++kk) {
-      const int k = c * kChunk + kk;
-      // rows beyond the layer's inputs carry zero weights; they read row 0 of the first segment
-      const float* rowp = (k < L.n_a) ? A + k * kT : ((k < L.n_a + L.n_b) ? B + (k - L.n_a) * kT : A);
-      const float4 a = *reinterpret_cast<const float4*>(rowp + 4 * sg);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float4 w4 = *reinterpret_cast<const float4*>(wc + kk * kW + 4 * cg + 64 * i);
-        const float wv[4] = {w4.x, w4.y, w4.z, w4.w};
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          acc[i][j][0] = fmaf(wv[j], a.x, acc[i][j][0]);
-          acc[i][j][1] = fmaf(wv[j], a.y, acc[i][j][1]);
-          acc[i][j][2] = fmaf(wv[j], a.z, acc[i][j][2]);
-          acc[i][j][3] = fmaf(wv[j], a.w, acc[i][j][3]);
-        }
-      }
-    }
-    cx.sync();  // chunk buffer free; after the last chunk: every thread is done reading the input segments
-  }
+  simt::gemm(cx, P.w + L.w_off, L.k_pad, A, L.n_a, B, L.n_b, smem + kOffW, acc);
 }
 
 // One CTA: tiles cx.block, cx.block + cx.nblocks, ...
@@ -350,10 +301,11 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
   }
 }
 
-// torch Linear weight [out][in] -> entry (k, c) of the packed [in padded][256] block
-__device__ __forceinline__ float pack_entry(const float* w, int n_in, int n_out, int k, int c) {
-  return (k < n_in && c < n_out) ? w[(size_t)c * n_in + k] : 0.f;
-}
+#ifdef __CUDACC__
+// colour output layer [3][256] + 3 biases as stored by torch, and the variance parameter (neus_simt.cu)
+__global__ void neus_pack_head_kernel(const float* __restrict__ wc, const float* __restrict__ bc, const float* __restrict__ variance,
+                                      float* __restrict__ dst_head, float* __restrict__ dst_var);
+#endif
 
 // ---------------------------------------------------------------------------------------------
 // host: layer table from the constructor arguments (neus.py:83-98)

@@ -1,4 +1,4 @@
-// NeuS field variant, training backward: CUDA thread context, weight packing and C ABI around the tile program of
+// NeuS field variant, training backward: kernel wrapper, weight packing and C ABI around the tile program of
 // neus_train_kernel.cuh (which is also compiled by g++ into a host emulation for the CPU tests).  One launch recomputes
 // the forward per 64-sample tile and walks back through the network, second order through the normal; it leaves the
 // operands of the weight-gradient GEMMs in global memory for neddf_wgrad / neddf_colsum_value_rows.
@@ -10,41 +10,10 @@
 namespace neddf {
 namespace neust {
 
-struct CudaCtx {
-  int tid, block, nblocks;
-  __device__ __forceinline__ void sync() { __syncthreads(); }
-  __device__ __forceinline__ void cp16(void* smem, const void* gmem) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
-  }
-  __device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-  __device__ __forceinline__ void cp_wait_1() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
-  __device__ __forceinline__ void cp_wait_0() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
-};
-
 __global__ void __launch_bounds__(kThreads, 1) neus_train_kernel(const __grid_constant__ Params T) {
   extern __shared__ __align__(16) float smem[];
-  CudaCtx cx{(int)threadIdx.x, (int)blockIdx.x, (int)gridDim.x};
+  simt::CudaCtx cx{(int)threadIdx.x, (int)blockIdx.x, (int)gridDim.x};
   tile_program(cx, T, smem);
-}
-
-// forward pack [k_pad][256] + bias [256] of one torch nn.Linear ([out][in], [out]) and, if dst_wt, its transposed pack
-// [256][256] over the input channels c0 .. c0 + 255
-__global__ void neus_train_pack_kernel(const float* __restrict__ w, const float* __restrict__ b, int n_in, int n_out, int k_pad,
-                                       int c0, float* __restrict__ dst_w, float* __restrict__ dst_b, float* __restrict__ dst_wt) {
-  const int stride = gridDim.x * blockDim.x, t0 = blockIdx.x * blockDim.x + threadIdx.x;
-  for (int idx = t0; idx < k_pad * kW; idx += stride) dst_w[idx] = neus::pack_entry(w, n_in, n_out, idx / kW, idx % kW);
-  if (dst_wt)
-    for (int idx = t0; idx < kW * kW; idx += stride) dst_wt[idx] = pack_t(w, n_in, n_out, c0, idx / kW, idx % kW);
-  if (blockIdx.x == 0)
-    for (int c = threadIdx.x; c < kW; c += blockDim.x) dst_b[c] = c < n_out ? b[c] : 0.f;
-}
-
-// colour output layer [3][256] + 3 biases as stored by torch, and the variance parameter
-__global__ void neus_train_pack_head_kernel(const float* __restrict__ wc, const float* __restrict__ bc, const float* __restrict__ variance,
-                                            float* __restrict__ dst_head, float* __restrict__ dst_var) {
-  for (int i = threadIdx.x; i < 3 * kW; i += blockDim.x) dst_head[i] = wc[i];
-  if (threadIdx.x < 3) dst_head[3 * kW + threadIdx.x] = bc[threadIdx.x];
-  if (threadIdx.x == 0) dst_var[0] = variance[0];
 }
 
 }  // namespace neust
@@ -98,11 +67,11 @@ extern "C" int32_t neddf_neus_train_set_weights(neddf_neus_train_t* h, const flo
     const neus::Layer& ly = sdf ? P.lsdf[l] : P.lcol[l];
     float* wt = sdf ? (l > 0 ? h->d_w + T.wt_sdf[l] : nullptr) : h->d_w + T.wt_col[l];
     const int c0 = (!sdf && l == 0) ? T.n_x : 0;
-    neust::neus_train_pack_kernel<<<64, 256, 0, s>>>(d_w[t], d_b[t], h->shape_in[t], h->shape_out[t], ly.k_pad, c0, h->d_w + ly.w_off,
-                                                    h->d_w + ly.b_off, wt);
+    simt::pack_linear_kernel<<<64, 256, 0, s>>>(d_w[t], d_b[t], h->shape_in[t], h->shape_out[t], ly.k_pad, wt ? neus::kW : 0, c0,
+                                                h->d_w + ly.w_off, h->d_w + ly.b_off, wt);
     NEDDF_LAUNCH_CHECK();
   }
-  neust::neus_train_pack_head_kernel<<<1, 256, 0, s>>>(d_w[n_layers - 1], d_b[n_layers - 1], d_variance, h->d_w + P.head_off, h->d_w + P.var_off);
+  neus::neus_pack_head_kernel<<<1, 256, 0, s>>>(d_w[n_layers - 1], d_b[n_layers - 1], d_variance, h->d_w + P.head_off, h->d_w + P.var_off);
   NEDDF_LAUNCH_CHECK();
   h->packed = true;
   return NEDDF_OK;

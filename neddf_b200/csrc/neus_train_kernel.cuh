@@ -40,6 +40,7 @@ using neus::kSub;
 using neus::kT;
 using neus::kThreads;
 using neus::kW;
+using simt::pack_t;
 
 struct Params {
   neus::Params f;           // network (forward packs, layer table) and sample geometry; f's outputs are unused
@@ -452,12 +453,6 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& T, float* sm
     }
     // (the trailing barrier protects X, H, F, geo, sdfv, up, gh, gn against the next tile)
   }
-}
-
-// torch Linear weight [out][in] -> entry (k = output channel, c) of a transposed pack [256][256] over the input channels
-// c0 .. c0 + 255 (the h part of an SDF / colour layer: c0 = 0; the F part of colour layer 0: c0 = n_x)
-__device__ __forceinline__ float pack_t(const float* w, int n_in, int n_out, int c0, int k, int c) {
-  return (k < n_out && c0 + c < n_in) ? w[(size_t)k * n_in + c0 + c] : 0.f;
 }
 
 // fills T.f (the forward program) and the transposed packs; returns the floats of the packed weight buffer

@@ -1,6 +1,6 @@
-// Sanitizer driver for the emulated NeRF training-backward kernel (TEST INFRASTRUCTURE): see neus_emul_main.cpp.
-// Exact-size buffers (a store past sample n - 1 is a heap overflow), full + ragged tiles, two CTAs, explicit samples
-// and fused ray geometry.  Exit code 0 = clean.
+// Sanitizer driver for the emulated NeRF forward and training-backward kernels (TEST INFRASTRUCTURE): see
+// neus_emul_main.cpp.  Exact-size buffers (a store past sample n - 1 is a heap overflow), full + ragged tiles, two CTAs,
+// explicit samples and fused ray geometry.  Exit code 0 = clean.
 #include "nerf_train_emul.cpp"
 
 #include <stdio.h>
@@ -8,8 +8,8 @@
 #include <random>
 
 static int run(const neddf_nerf_config_t& cfg, int n, bool rays, unsigned seed) {
-  int sin[nerft::kMaxLayers + 3], sout[nerft::kMaxLayers + 3];
-  const int nl = nerft::layer_shapes(&cfg, sin, sout);
+  int sin[nerf::kMaxLayers + 3], sout[nerf::kMaxLayers + 3];
+  const int nl = nerf::layer_shapes(&cfg, sin, sout);
   const int L = cfg.layer_count, n_e = 6 * cfg.embed_pos_rank, n_d = 6 * cfg.embed_dir_rank;
   std::mt19937 g(seed);
   std::normal_distribution<float> nd(0.f, 1.f);
@@ -41,6 +41,14 @@ static int run(const neddf_nerf_config_t& cfg, int n, bool rays, unsigned seed) 
     ro[3 * i] = 0.1f * nd(g); ro[3 * i + 1] = 0.1f * nd(g); ro[3 * i + 2] = 0.1f * nd(g);
     for (int j = 0; j < n_edges; ++j) dists[(size_t)i * n_edges + j] = 2.f + 0.5f * j + 0.1f * fabsf(nd(g));
   }
+  std::vector<float> density(total), color(3 * total);
+  const int rc_f = nerf_emul_forward(&cfg, wp.data(), bp.data(), nl, lowpass, rays ? nullptr : pos.data(), rays ? nullptr : dir.data(),
+                                     rays ? nullptr : var.data(), rays ? rd.data() : nullptr, rays ? ro.data() : nullptr,
+                                     rays ? dists.data() : nullptr, n, n_edges, NEDDF_SAMPLING_CONE, 2.6e-4f, density.data(), color.data(), 2);
+  double sum_f = 0;
+  for (float v : density) sum_f += v;
+  for (float v : color) sum_f += v;
+  printf("forward rc %d checksum %.6f (%lld samples)\n", rc_f, sum_f, total);
   std::vector<float> gd(total), gc(3 * total);
   for (auto& v : gd) v = nd(g);
   for (auto& v : gc) v = nd(g);
@@ -54,8 +62,8 @@ static int run(const neddf_nerf_config_t& cfg, int n, bool rays, unsigned seed) 
   for (float v : G) sum += v;
   for (float v : GC1) sum += v;
   for (float v : GZD) sum += v;
-  printf("rc %d checksum %.6f (%lld samples)\n", rc, sum, total);
-  return (rc == 0 && sum == sum) ? 0 : 1;
+  printf("backward rc %d checksum %.6f (%lld samples)\n", rc, sum, total);
+  return (rc_f == 0 && sum_f == sum_f && rc == 0 && sum == sum) ? 0 : 1;
 }
 
 int main() {

@@ -25,14 +25,10 @@ extern "C" int neus_emul_forward(const neddf_neus_config_t* cfg, const float* co
   int sin[neus::kMaxSdf + neus::kMaxCol + 2], sout[neus::kMaxSdf + neus::kMaxCol + 2];
   if (neus::layer_shapes(cfg, sin, sout) != n_layers) return -2;
   std::vector<float> packed(w_floats, 0.f);
-  // neddf_neus_set_weights: neus_pack_kernel per layer, neus_pack_head_kernel
+  // neddf_neus_set_weights: simt::pack_linear_kernel per layer, neus_pack_head_kernel
   for (int t = 0; t < n_layers - 1; ++t) {
     const neus::Layer& ly = (t < P.n_sdf) ? P.lsdf[t] : P.lcol[t - P.n_sdf];
-    for (int idx = 0; idx < ly.k_pad * neus::kW; ++idx) {
-      const int k = idx / neus::kW, c = idx - k * neus::kW;
-      packed[ly.w_off + idx] = neus::pack_entry(w[t], sin[t], sout[t], k, c);
-    }
-    for (int c = 0; c < neus::kW; ++c) packed[ly.b_off + c] = c < sout[t] ? b[t][c] : 0.f;
+    simt::pack_linear(0, 1, w[t], b[t], sin[t], sout[t], ly.k_pad, 0, 0, &packed[ly.w_off], &packed[ly.b_off], nullptr);
   }
   for (int i = 0; i < 3 * neus::kW; ++i) packed[P.head_off + i] = w[n_layers - 1][i];
   for (int i = 0; i < 3; ++i) packed[P.head_off + 3 * neus::kW + i] = b[n_layers - 1][i];

@@ -22,19 +22,14 @@ extern "C" int neus_train_emul(const neddf_neus_config_t* cfg, const float* cons
   int sin[neus::kMaxSdf + neus::kMaxCol + 2], sout[neus::kMaxSdf + neus::kMaxCol + 2];
   if (neus::layer_shapes(cfg, sin, sout) != n_layers) return -2;
   std::vector<float> packed(w_floats, 0.f);
-  // neddf_neus_train_set_weights: neus_train_pack_kernel per layer, neus_train_pack_head_kernel
+  // neddf_neus_train_set_weights: simt::pack_linear_kernel per layer, neus_pack_head_kernel
   for (int t = 0; t < n_layers - 1; ++t) {
     const bool sdf = t < P.n_sdf;
     const int l = sdf ? t : t - P.n_sdf;
     const neus::Layer& ly = sdf ? P.lsdf[l] : P.lcol[l];
-    for (int idx = 0; idx < ly.k_pad * neus::kW; ++idx)
-      packed[ly.w_off + idx] = neus::pack_entry(w[t], sin[t], sout[t], idx / neus::kW, idx % neus::kW);
-    const int wt = sdf ? (l > 0 ? T.wt_sdf[l] : -1) : T.wt_col[l];
+    float* wt = sdf ? (l > 0 ? &packed[T.wt_sdf[l]] : nullptr) : &packed[T.wt_col[l]];
     const int c0 = (!sdf && l == 0) ? T.n_x : 0;
-    if (wt >= 0)
-      for (int idx = 0; idx < neus::kW * neus::kW; ++idx)
-        packed[wt + idx] = neust::pack_t(w[t], sin[t], sout[t], c0, idx / neus::kW, idx % neus::kW);
-    for (int c = 0; c < neus::kW; ++c) packed[ly.b_off + c] = c < sout[t] ? b[t][c] : 0.f;
+    simt::pack_linear(0, 1, w[t], b[t], sin[t], sout[t], ly.k_pad, wt ? neus::kW : 0, c0, &packed[ly.w_off], &packed[ly.b_off], wt);
   }
   for (int i = 0; i < 3 * neus::kW; ++i) packed[P.head_off + i] = w[n_layers - 1][i];
   for (int i = 0; i < 3; ++i) packed[P.head_off + 3 * neus::kW + i] = b[n_layers - 1][i];

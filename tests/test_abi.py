@@ -61,6 +61,65 @@ def test_layer_shapes_and_validation(built):
     assert b"256" in lib.neddf_last_error()
 
 
+def test_nerf_structure_limits_are_refused_before_any_launch(built):
+    """The configuration checks of the two NeRF handles at their boundaries.  A refused structure returns the code its
+    entry point has always returned, before any CUDA call.  An accepted one gets as far as allocating its packed weights
+    (NEDDF_OK with a GPU, NEDDF_E_CUDA without one).  neddf_nerf_layer_shapes checks the layer count only."""
+    import ctypes as C
+
+    from neddf_b200 import _lib as L
+    lib = L.lib()
+    OK, INVALID, CUDA, UNSUPPORTED = 0, -1, -2, -3
+    accepted = (OK, CUDA)
+
+    def cfg(layer_count=8, pos=10, dirs=4, skips=(4,), act=1, density_act=1):
+        c = L.NerfConfig()
+        c.embed_pos_rank, c.embed_dir_rank, c.layer_count, c.layer_width = pos, dirs, layer_count, 256
+        c.activation_type, c.density_activation_type = act, density_act
+        c.n_skips = len(skips)
+        for i, v in enumerate(skips):
+            c.skips[i] = v
+        return c
+
+    def codes(**kw):
+        c = cfg(**kw)
+        out = [lib.neddf_nerf_layer_shapes(C.byref(c), None, 0)]
+        for create, destroy in ((lib.neddf_nerf_create, lib.neddf_nerf_destroy),
+                                (lib.neddf_nerf_train_create, lib.neddf_nerf_train_destroy)):
+            h = C.c_void_p()
+            rc = create(C.byref(c), C.byref(h))
+            assert (rc == OK) == bool(h.value)
+            if h.value:
+                destroy(h)
+            out.append("accepted" if rc in accepted else rc)
+        return tuple(out)
+
+    # layer_count: forward 2..13, training backward 2..12
+    assert codes(layer_count=1, skips=()) == (INVALID, UNSUPPORTED, UNSUPPORTED)
+    assert codes(layer_count=2, skips=()) == (5, "accepted", "accepted")
+    assert codes(layer_count=12) == (15, "accepted", "accepted")
+    assert codes(layer_count=13) == (16, "accepted", UNSUPPORTED)
+    assert b"2..12" in lib.neddf_last_error()
+    assert codes(layer_count=14) == (INVALID, UNSUPPORTED, UNSUPPORTED)
+    assert b"2..12" in lib.neddf_last_error()
+    c = cfg(layer_count=14)
+    assert lib.neddf_nerf_create(C.byref(c), C.byref(C.c_void_p())) == UNSUPPORTED
+    assert b"layer_count must be 2..13" in lib.neddf_last_error()
+    # embedding ranks: 6 * embed_pos_rank <= 64, 6 * embed_dir_rank <= 32
+    assert codes(pos=10) == (11, "accepted", "accepted")
+    assert codes(pos=11) == (11, UNSUPPORTED, UNSUPPORTED)
+    assert codes(dirs=5) == (11, "accepted", "accepted")
+    assert codes(dirs=6) == (11, UNSUPPORTED, UNSUPPORTED)
+    # a skip after the last hidden layer would widen the heads
+    assert codes(skips=(6,)) == (11, "accepted", "accepted")
+    assert codes(skips=(7,)) == (11, UNSUPPORTED, UNSUPPORTED)
+    assert b"skip" in lib.neddf_last_error()
+    # activation ids: a malformed one is an invalid argument to the forward
+    for kw in (dict(act=3), dict(density_act=-1)):
+        assert codes(**kw) == (11, INVALID, UNSUPPORTED), kw
+        assert b"bad activation" in lib.neddf_last_error()
+
+
 def test_entry_points_fail_loudly_without_a_gpu(built):
     """No CPU fallback: with no CUDA device (this container) creating a field returns an error code
     and a message, NULL arguments are rejected before any CUDA call, nothing crashes or leaks a handle."""

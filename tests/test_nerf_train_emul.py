@@ -1,7 +1,10 @@
-"""The NeRF variant's training-backward kernel (csrc/nerf_train.cu), executed on the CPU.
+"""The NeRF variant's kernels - the forward (csrc/nerf_simt.cu) and the training backward (csrc/nerf_train.cu) - executed
+on the CPU.
 
-Its tile program (neddf_b200/csrc/nerf_train_kernel.cuh) is compiled by g++ into tests/emul/libnerf_train_emul.so (a CTA =
-256 OS threads, pthread barrier for __syncthreads) and run on the samples and the upstream gradients (d loss / d density,
+Their tile programs (neddf_b200/csrc/nerf_kernel.cuh, nerf_train_kernel.cuh) are compiled by g++ into
+tests/emul/libnerf_train_emul.so (a CTA = 256 OS threads, pthread barrier for __syncthreads).  The forward is run against
+the goldens recorded from the REAL reference (tests/golden/make_nerf_golden.py).  The backward is run on the samples and
+the upstream gradients (d loss / d density,
 d loss / d colour per sample, captured with tensor hooks) of fixtures recorded from the REAL reference's autograd
 (tests/golden/make_nerf_train_golden.py).  The parameter gradients are then assembled exactly as the GPU path does -
 gW = X^T G over all samples, bias = column sums - with numpy standing in for neddf_wgrad, and compared with the
@@ -18,7 +21,8 @@ import pytest
 import torch
 
 from oracle import neddf_oracle as orc
-from tests.helpers import GOLDEN, assert_parity, nerr
+from tests.helpers import GOLDEN, PARITY_TOL, assert_parity, nerr
+from tests.test_nerf_oracle import NerfCase
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "emul", "nerf_train_emul.cpp")
@@ -55,13 +59,16 @@ class TrainCase:
 def emul():
     if shutil.which("g++") is None or not os.path.isdir(CUDA_INC):
         pytest.skip("g++ / CUDA headers not available")
-    deps = [SRC, os.path.join(HERE, "emul", "emul_common.h"), os.path.join(HERE, "..", "neddf_b200", "csrc", "nerf_train_kernel.cuh"),
-            os.path.join(HERE, "..", "neddf_b200", "csrc", "common.cuh"), os.path.join(HERE, "..", "include", "neddf_b200.h")]
+    csrc = os.path.join(HERE, "..", "neddf_b200", "csrc")
+    deps = [SRC, os.path.join(HERE, "emul", "emul_common.h"), os.path.join(HERE, "..", "include", "neddf_b200.h")] + \
+        [os.path.join(csrc, h) for h in ("nerf_train_kernel.cuh", "nerf_kernel.cuh", "simt_tile.cuh", "field_math.cuh", "field.cuh",
+                                         "common.cuh")]
     if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in deps):
         subprocess.run(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-pthread", "-I" + CUDA_INC, SRC, "-o", LIB],
                        check=True)
     lib = C.CDLL(LIB)
     lib.nerf_train_emul.restype = C.c_int
+    lib.nerf_emul_forward.restype = C.c_int
     return lib
 
 
@@ -103,6 +110,88 @@ def run_backward(lib, nc, alpha, ws, bs, ray_dir, ray_orig, dists, sampling_type
     assert rc == 0
     assert all(np.isfinite(v).all() for v in buf.values())
     return buf, gd, gc
+
+
+def run_forward(lib, nc, alpha, ws, bs, samples=None, rays=None, sampling_type="cone", nblocks=2):
+    """The emulated forward kernel on explicit samples ((pos, dirs, var), each [..., 3]) or rays ((ray_dir, ray_orig,
+    dists), fused geometry); returns density [n] and colour [n, 3], from NaN-filled buffers."""
+    def p(a):
+        return None if a is None else a.ctypes.data_as(FP)
+
+    def f32(t):
+        return np.ascontiguousarray(t.numpy(), np.float32)
+
+    pos = dirs = var = rd = ro = di = None
+    if rays is not None:
+        rd, ro, di = (f32(t) for t in rays)
+        n_arg, S = di.shape  # rays, edges per ray
+        n = n_arg * S
+    else:
+        pos, dirs, var = (f32(t).reshape(-1, 3) for t in samples)
+        n = n_arg = pos.shape[0]
+        S = 0
+    density, color = np.full((n,), np.nan, np.float32), np.full((n, 3), np.nan, np.float32)
+    lowpass = orc.lowpass_scale(nc.embed_pos_rank, alpha).numpy().astype(np.float32)
+    wp = (FP * len(ws))(*[p(a) for a in ws])
+    bp = (FP * len(bs))(*[p(a) for a in bs])
+    cfg = cfg_struct(nc)
+    radius = orc.CONE_RAY_RADIUS if sampling_type == "cone" else 0.0
+    rc = lib.nerf_emul_forward(C.byref(cfg), wp, bp, len(ws), p(lowpass), p(pos), p(dirs), p(var), p(rd), p(ro), p(di), C.c_longlong(n_arg),
+                               C.c_int(S), C.c_int({"point": 0, "cone": 1}[sampling_type]), C.c_float(radius), p(density), p(color),
+                               C.c_int(nblocks))
+    assert rc == 0
+    assert np.isfinite(density).all() and np.isfinite(color).all()  # every sample written
+    return density, color
+
+
+def torch_layout_weights(c: NerfCase, tag):
+    """[out,in] weights and [out] biases of a pass's network, in the order of neddf_nerf_layer_shapes."""
+    pre = f"w_{tag}." if f"w_{tag}.layers.0.weight" in c.z else "w_fine."
+    names = [n for n, _, _ in orc.nerf_layer_shapes(c.nc)]
+    return [np.ascontiguousarray(c.z[pre + n + ".weight"], np.float32) for n in names], \
+        [np.ascontiguousarray(c.z[pre + n + ".bias"], np.float32) for n in names]
+
+
+@pytest.mark.parametrize("name", ["relu", "tanhexp"])
+def test_emulated_forward_matches_reference(emul, name):
+    """Per-sample field outputs of both passes, with explicit samples and with the fused ray geometry, against the real
+    reference's (the bound of the GPU test, tests/test_nerf_gpu.py)."""
+    c = NerfCase(name)
+    d, o = orc.make_rays(c.t("uv"), c.cam)
+    for tag, dists in (("coarse", orc.coarse_dists(c.rc, c.t("u_coarse"))), ("fine", c.t("dists_fine"))):
+        ws, bs = torch_layout_weights(c, tag)
+        pos, dd, var = orc.make_samples(c.rc, d, o, dists)
+        outs = {"explicit": run_forward(emul, c.nc, c.alpha, ws, bs, samples=(pos, dd, var), sampling_type=c.rc.sampling_type),
+                "fused": run_forward(emul, c.nc, c.alpha, ws, bs, rays=(d, o, dists), sampling_type=c.rc.sampling_type)}
+        for how, (dens, col) in outs.items():
+            for k, v in (("density", dens), ("color", col)):
+                ref = c.z[f"field_{tag}_{k}"]
+                assert nerr(v.reshape(ref.shape), ref) < PARITY_TOL, (tag, k, how)
+
+
+def test_emulated_forward_ragged_tiles(emul):
+    """Sample counts that are not multiples of the 64-sample tile, and more tiles than CTAs, against the oracle: the
+    ReLU golden's network, and a LeakyReLU network with three skips."""
+    c = NerfCase("relu")
+    leaky = orc.NerfConfig(embed_pos_rank=4, embed_dir_rank=2, layer_count=5, activation_type="LeakyReLU",
+                           density_activation_type="LeakyReLU", skips=[0, 1, 3], lowpass_alpha_offset=2.0)
+    P = orc.nerf_init_params(leaky, 11)
+    names = [n for n, _, _ in orc.nerf_layer_shapes(leaky)]
+    nets = [(c.nc, c.alpha, c.params("fine"), *torch_layout_weights(c, "fine")),
+            (leaky, leaky.lowpass_alpha_at(700), P, [np.ascontiguousarray(P[n + ".weight"].t().numpy()) for n in names],
+             [np.ascontiguousarray(P[n + ".bias"].numpy()) for n in names])]
+    g = torch.Generator().manual_seed(5)
+    for nc, alpha, params, ws, bs in nets:
+        for n in (1, 63, 65, 300):
+            pos = torch.rand(1, n, 3, generator=g) * 2 - 1
+            dd = torch.nn.functional.normalize(torch.randn(1, n, 3, generator=g), dim=-1)
+            var = torch.rand(1, n, 3, generator=g) * 1e-3
+            dens, col = run_forward(emul, nc, alpha, ws, bs, samples=(pos, dd, var), nblocks=2)
+            with torch.no_grad():
+                ref = orc.nerf_forward(params, nc, alpha, pos, dd, var)
+            for k, v in (("density", dens), ("color", col)):
+                r = ref[k].numpy().reshape(v.shape)
+                assert np.abs(v - r).max() <= PARITY_TOL * max(np.abs(r).max(), 1.0), (nc.activation_type, n, k)
 
 
 def oracle_grads(c: TrainCase, dtype):
@@ -369,12 +458,12 @@ def _san_build(tmp_path, name, flags):
 
 def test_emulated_backward_under_sanitizers(emul, tmp_path):
     """AddressSanitizer + UBSan (memcheck: exact-size buffers, float4 alignment) and ThreadSanitizer (racecheck, best
-    effort) on the emulated training-backward kernel (the negative controls that show the detectors see this kind of code
+    effort) on the emulated forward and training-backward kernels (the negative controls that show the detectors see this kind of code
     live in tests/test_neus_emul.py: same harness, same GEMM loop)."""
     env = dict(os.environ, TSAN_OPTIONS="halt_on_error=0 exitcode=66", ASAN_OPTIONS="detect_leaks=0")
     r = subprocess.run([_san_build(tmp_path, "asan", ["-fsanitize=address,undefined", "-fno-sanitize-recover=all"])], capture_output=True,
                        text=True, env=env, timeout=600)
     assert r.returncode == 0 and "runtime error" not in r.stderr and "AddressSanitizer" not in r.stderr, r.stderr[-1500:]
-    assert r.stdout.count("rc 0 checksum") == 2
+    assert r.stdout.count("forward rc 0 checksum") == 2 and r.stdout.count("backward rc 0 checksum") == 2
     r = subprocess.run([_san_build(tmp_path, "tsan", ["-fsanitize=thread"])], capture_output=True, text=True, env=env, timeout=600)
     assert r.returncode == 0 and "ThreadSanitizer" not in r.stderr, r.stderr[-1500:]
