@@ -503,6 +503,42 @@ int32_t neddf_mc_normals(const float* d_volume, int32_t n0, int32_t n1, int32_t 
                          void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Narrow-band marching cubes on an n^3 grid, n in [2, 2048] (csrc/mcubes_band.cu): the dense rule and case table
+ * above, evaluated only in bricks of 8^3 cells near the level set.  nb = ceil((n - 1) / 8) bricks per axis; brick b
+ * covers grid points [8b, min(8b + 8, n - 1)] per axis.  The caller evaluates the field between the calls:
+ *   neddf_mcb_points   d_active NULL: the int32 grid indices (i, j, k) of points [first, first + count) of the
+ *                      (nb + 1)^3 brick corners (corner c is min(8c, n - 1) per axis); otherwise of the 729 points of
+ *                      each listed brick (local point l is min(8b + l, n - 1): partial bricks clamped).  d_idx [count,3].
+ *   neddf_mcb_bricks   d_corner_values [(nb + 1)^3] -> a brick is active if a corner is non-finite or all 8 satisfy
+ *                      |v - threshold| <= band (fp32).  d_slot int32 [nb^3] (slot of the brick, -1 inactive),
+ *                      d_active int32 [nb^3] (the first A entries: active bricks, ascending), d_count int64 [1] = A.
+ *   neddf_mcb_count    d_values [A * 729] at the active bricks' points -> d_totals[0] = V, d_totals[1] = F.
+ *                      NEDDF_E_UNSUPPORTED if A * 2187 or A * 512 * 5 does not fit int32.
+ *   neddf_mcb_emit     d_vertices [V,3] and d_faces [F,3] in the dense kernels' order: vertices by (grid point,
+ *                      axis), faces by (cube, table order); vertex arithmetic as neddf_mc_emit on global indices.
+ *   neddf_mcb_normals  (optional, after emit) d_normals [V,3] by neddf_mc_normals' rule; cubes in inactive bricks
+ *                      contribute nothing.
+ * If every brick that holds an emitting cube of the dense grid is active, the outputs equal neddf_mc_* on the dense
+ * volume bit for bit.  The count workspace (neddf_mcb_workspace_bytes) is shared by count, emit and normals; the
+ * emit workspace (neddf_mcb_emit_workspace_bytes, sized from V and F) by emit and normals.
+ * ------------------------------------------------------------------------------------------------ */
+int32_t neddf_mcb_points(const int32_t* d_active, int32_t n, int64_t first, int64_t count, int32_t* d_idx, void* stream);
+int64_t neddf_mcb_bricks_workspace_bytes(int32_t n);
+int32_t neddf_mcb_bricks(const float* d_corner_values, int32_t n, float threshold, float band, void* d_workspace,
+                         int32_t* d_slot, int32_t* d_active, int64_t* d_count, void* stream);
+int64_t neddf_mcb_workspace_bytes(int32_t n, int64_t n_active);
+int32_t neddf_mcb_count(const float* d_values, int32_t n, float threshold, const int32_t* d_slot,
+                        const int32_t* d_active, int64_t n_active, void* d_workspace, int64_t* d_totals, void* stream);
+int64_t neddf_mcb_emit_workspace_bytes(int64_t n_vertices, int64_t n_faces);
+int32_t neddf_mcb_emit(const float* d_values, int32_t n, float threshold, const int32_t* d_slot,
+                       const int32_t* d_active, int64_t n_active, const void* d_workspace, int64_t n_vertices,
+                       int64_t n_faces, void* d_emit_workspace, float* d_vertices, int64_t* d_faces, void* stream);
+int32_t neddf_mcb_normals(const float* d_values, int32_t n, const int32_t* d_slot, const int32_t* d_active,
+                          int64_t n_active, const void* d_workspace, int64_t n_vertices, int64_t n_faces,
+                          const void* d_emit_workspace, const float* d_vertices, const int64_t* d_faces,
+                          float* d_normals, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Sphere tracing of a level set (csrc/surface.cu; no reference function is replaced - the reference shows its
  * surfaces only through volumetric renders and its Open3D visualiser).  Per ray g(t) = field(o + t d) - level;
  * stepping t += g is safe where |dD/dt| <= 1, which NeDDF trains (constraints_dDdt, neddf/network/neddf.py:271).

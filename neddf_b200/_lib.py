@@ -125,6 +125,14 @@ _SIGNATURES = {
     "neddf_mc_count": (_I32, [_P, _I32, _I32, _I32, _F, _P, _P, _P]),
     "neddf_mc_emit": (_I32, [_P, _I32, _I32, _I32, _F, _P, _P, _P, _P]),
     "neddf_mc_normals": (_I32, [_P, _I32, _I32, _I32, _F, _P, _P, _P, _P, _P]),
+    "neddf_mcb_points": (_I32, [_P, _I32, _I64, _I64, _P, _P]),
+    "neddf_mcb_bricks_workspace_bytes": (_I64, [_I32]),
+    "neddf_mcb_bricks": (_I32, [_P, _I32, _F, _F, _P, _P, _P, _P, _P]),
+    "neddf_mcb_workspace_bytes": (_I64, [_I32, _I64]),
+    "neddf_mcb_count": (_I32, [_P, _I32, _F, _P, _P, _I64, _P, _P, _P]),
+    "neddf_mcb_emit_workspace_bytes": (_I64, [_I64, _I64]),
+    "neddf_mcb_emit": (_I32, [_P, _I32, _F, _P, _P, _I64, _P, _I64, _I64, _P, _P, _P, _P]),
+    "neddf_mcb_normals": (_I32, [_P, _I32, _P, _P, _I64, _P, _I64, _I64, _P, _P, _P, _P, _P]),
     "neddf_trace_init": (_I32, [_P, _P, _I64, _F] + [_P] * 8 + [_P]),
     "neddf_trace_step": (_I32, [_P, _P, _I64, _P, _P, _F, _F, _I32] + [_P] * 9 + [_P]),
     "neddf_trace_hits": (_I32, [_P, _P, _I64, _P, _P, _P, _P, _P, _P, _P]),

@@ -13,6 +13,7 @@
 
 #include "common.cuh"
 #include "mc_table.cuh"
+#include "mc_vertex.cuh"
 
 namespace neddf {
 namespace {
@@ -86,14 +87,7 @@ __global__ void __launch_bounds__(kMcThreads) mc_vertices(const float* __restric
   const int g = s / 3, axis = s - 3 * g;
   const int k = g % n2, r = g / n2, j = r % n1, i = r / n1;
   const int step = axis == 0 ? n1 * n2 : (axis == 1 ? n2 : 1);
-  const float v0 = vol[g], v1 = vol[g + step];
-  const float t = __fdiv_rn(__fsub_rn(thr, v0), __fsub_rn(v1, v0));
-  float p[3] = {(float)i, (float)j, (float)k};
-  p[axis] = __fadd_rn(p[axis], t);
-  float* out = vertices + 3 * (int64_t)id;
-  out[0] = p[0];
-  out[1] = p[1];
-  out[2] = p[2];
+  mc::edge_vertex(thr, vol[g], vol[g + step], (float)i, (float)j, (float)k, axis, vertices + 3 * (int64_t)id);
 }
 
 __global__ void __launch_bounds__(kMcThreads) mc_faces(int n0, int n1, int n2, const uint8_t* __restrict__ cases,
@@ -149,30 +143,12 @@ __global__ void __launch_bounds__(kMcThreads) mc_normals(const float* __restrict
         const int64_t* fv = faces + 3 * (int64_t)f;
         const int64_t i0 = fv[0], i1 = fv[1], i2 = fv[2];
         if (i0 != id && i1 != id && i2 != id) continue;
-        const float* p0 = vertices + 3 * i0;
-        const float* p1 = vertices + 3 * i1;
-        const float* p2 = vertices + 3 * i2;
-        const float ax = __fsub_rn(p1[0], p0[0]), ay = __fsub_rn(p1[1], p0[1]), az = __fsub_rn(p1[2], p0[2]);
-        const float bx = __fsub_rn(p2[0], p0[0]), by = __fsub_rn(p2[1], p0[1]), bz = __fsub_rn(p2[2], p0[2]);
-        nx = __fadd_rn(nx, __fsub_rn(__fmul_rn(ay, bz), __fmul_rn(az, by)));
-        ny = __fadd_rn(ny, __fsub_rn(__fmul_rn(az, bx), __fmul_rn(ax, bz)));
-        nz = __fadd_rn(nz, __fsub_rn(__fmul_rn(ax, by), __fmul_rn(ay, bx)));
+        mc::add_face_normal(vertices + 3 * i0, vertices + 3 * i1, vertices + 3 * i2, nx, ny, nz);
       }
     }
   }
-  const float len = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(nx, nx), __fmul_rn(ny, ny)), __fmul_rn(nz, nz)));
-  float* out = normals + 3 * (int64_t)id;
-  if (len == 0.0f) {
-    const int step = axis == 0 ? n1 * n2 : (axis == 1 ? n2 : 1);
-    const float sign = vol[g + step] > vol[g] ? 1.0f : -1.0f;
-    out[0] = axis == 0 ? sign : 0.0f;
-    out[1] = axis == 1 ? sign : 0.0f;
-    out[2] = axis == 2 ? sign : 0.0f;
-    return;
-  }
-  out[0] = __fdiv_rn(nx, len);
-  out[1] = __fdiv_rn(ny, len);
-  out[2] = __fdiv_rn(nz, len);
+  const int step = axis == 0 ? n1 * n2 : (axis == 1 ? n2 : 1);
+  mc::finish_normal(nx, ny, nz, axis, vol[g], vol[g + step], normals + 3 * (int64_t)id);
 }
 
 int32_t check_dims(int32_t n0, int32_t n1, int32_t n2, const char* who) {

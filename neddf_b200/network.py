@@ -11,6 +11,7 @@ update them in place).
 """
 import contextlib
 import ctypes as C
+import math
 import warnings
 from typing import Dict, List, Optional, Tuple
 
@@ -288,17 +289,42 @@ class BaseNeuralField(nn.Module):
         n = int(cube_resolution)
         device = self.device
         with torch.set_grad_enabled(False):
-            ids = torch.from_numpy(np.linspace(-cube_range, cube_range, n).astype(np.float32)).to(device)
+            ids = self._grid_ids(cube_range, n)
             total = n ** 3
             out = torch.empty(total, dtype=torch.float32, device=device)
-            one_dir = torch.tensor([1.0, 0.0, 0.0], device=device)
             for i in range(0, total, chunk):
                 j = min(total, i + chunk)
                 lin = torch.arange(i, j, device=device)
-                p = torch.stack([ids[lin % n], ids[lin // (n * n)], ids[(lin // n) % n]], 1)[None]
-                s = Sampling(p, one_dir.expand(j - i, 3)[None].contiguous(), torch.zeros_like(p))
-                out[i:j] = self.forward(s)[field_name].reshape(-1)
+                out[i:j] = self._grid_values(field_name, ids, torch.stack([lin // (n * n), (lin // n) % n, lin % n], 1))
             return out.view(n, n, n)
+
+    def _grid_ids(self, cube_range: float, n: int) -> Tensor:
+        """``voxelize``'s axis coordinates ``linspace(-r, r, n)`` in fp32, on the module's device."""
+        return torch.from_numpy(np.linspace(-cube_range, cube_range, n).astype(np.float32)).to(self.device)
+
+    def _grid_values(self, field_name: str, ids: Tensor, idx: Tensor) -> Tensor:
+        """The field at grid points ``idx`` [m, 3] (i, j, k) of ``voxelize``'s grid, [m] fp32: the point (x, y, z) =
+        (ids[k], ids[i], ids[j]) gathered on the device, direction (1, 0, 0), zero variance, one ``forward``."""
+        p = torch.stack([ids[idx[:, 2]], ids[idx[:, 0]], ids[idx[:, 1]]], 1)[None]
+        dirs = torch.zeros_like(p)
+        dirs[..., 0] = 1.0
+        return self.forward(Sampling(p, dirs, torch.zeros_like(p)))[field_name].reshape(-1)
+
+    def _band_mesh(self, field_name: str, threshold: float, cube_range: float, n: int, lipschitz: float,
+                   normals: bool, chunk: int = 65536):
+        """``narrow_band_marching_cubes`` over ``voxelize``'s grid, the points evaluated by ``_grid_values`` in chunks
+        of ``chunk`` as ``_grid_volume`` evaluates them; band = L sqrt(3) 8 h in float64, rounded to fp32."""
+        from .mesh import BRICK, narrow_band_marching_cubes
+        h = 2.0 * float(cube_range) / (n - 1)
+        band = float(np.float32(lipschitz * math.sqrt(3.0) * BRICK * h))
+        with torch.set_grad_enabled(False), torch.cuda.device(self.device):
+            ids = self._grid_ids(cube_range, n)
+
+            def evaluate(idx: Tensor) -> Tensor:
+                return torch.cat([self._grid_values(field_name, ids, idx[i:i + chunk])
+                                  for i in range(0, idx.shape[0], chunk)])
+
+            return narrow_band_marching_cubes(evaluate, n, threshold, band, normals=normals)
 
     # field -> sign of the colour pass's view direction relative to the vertex normal (which points toward increasing
     # value): -1 for a field that grows outward, +1 for one that grows inward, so the surface is seen from outside.
@@ -306,7 +332,7 @@ class BaseNeuralField(nn.Module):
     _MESH_VIEW_SIGN: Dict[str, float] = {}
 
     def extract_mesh(self, field_name: str, threshold: float, cube_range: float = 1.1, cube_resolution: int = 64,
-                     with_color: bool = False):
+                     with_color: bool = False, lipschitz: Optional[float] = None):
         """Triangle mesh of the level set ``field == threshold`` over ``voxelize``'s grid, on the module's device:
         (vertices [V,3] fp32, faces [F,3] int64).
 
@@ -323,20 +349,43 @@ class BaseNeuralField(nn.Module):
         ``+normal`` for ``density`` (NeDDF, NeRF).  Any other field raises ValueError.  Vertices and faces are the
         ``with_color=False`` ones bit for bit.
 
+        ``lipschitz=L`` (finite, > 0; only the network's distance field, ``distance`` for NeDDF and ``sdf`` for NeuS)
+        evaluates the grid only in a narrow band around the level set (``neddf_b200.mesh.narrow_band_marching_cubes``
+        with band ``L sqrt(3) 8 h``), and ``cube_resolution`` may then be up to 2048.  If the field is L-Lipschitz on
+        the grid, the result is the dense call's (``lipschitz=None``) bit for bit, in the same order; the bound is the
+        caller's claim about its field and is not checked.
+
         The reference's visualiser writes its mesh in a scaled, half-voxel-shifted index space instead
         (fields_visualizer.py:546-547); that frame is not reproduced here."""
-        from .mesh import marching_cubes
+        from .mesh import BAND_MAX_DIM, MAX_DIM, marching_cubes
         n = int(cube_resolution)
         if n < 2:
             raise ValueError("extract_mesh: cube_resolution must be >= 2")
         if with_color and field_name not in self._MESH_VIEW_SIGN:
             raise ValueError(f"extract_mesh: with_color needs a field that is monotone across the surface; "
                              f"{type(self).__name__} supports {sorted(self._MESH_VIEW_SIGN)}, got {field_name!r}")
-        volume = self._grid_volume(field_name, cube_range, n)
-        if with_color:
-            vertices, faces, index_normals = marching_cubes(volume, threshold, normals=True)
+        if lipschitz is not None:
+            lipschitz = float(lipschitz)
+            if not (math.isfinite(lipschitz) and lipschitz > 0):
+                raise ValueError(f"extract_mesh: lipschitz must be finite and > 0, got {lipschitz!r}")
+            if self._TRACE_FIELD is None or field_name != self._TRACE_FIELD:
+                raise ValueError(f"extract_mesh: the narrow band needs a distance field; {type(self).__name__} "
+                                 f"{'has none' if self._TRACE_FIELD is None else 'has ' + repr(self._TRACE_FIELD)}, "
+                                 f"got {field_name!r}")
+            if n > BAND_MAX_DIM:
+                raise ValueError(f"extract_mesh: cube_resolution must be in [2, {BAND_MAX_DIM}] with lipschitz, "
+                                 f"got {n}")
+            mesh = self._band_mesh(field_name, threshold, cube_range, n, lipschitz, with_color)
         else:
-            vertices, faces = marching_cubes(volume, threshold)
+            if n > MAX_DIM:
+                raise ValueError(f"extract_mesh: cube_resolution above {MAX_DIM} needs the narrow band: pass "
+                                 f"lipschitz (a bound on the field's gradient norm), got {n}")
+            volume = self._grid_volume(field_name, cube_range, n)
+            mesh = marching_cubes(volume, threshold, normals=with_color)
+        if with_color:
+            vertices, faces, index_normals = mesh
+        else:
+            vertices, faces = mesh
         h = 2.0 * float(cube_range) / (n - 1)
         v = vertices.double()
         r = float(cube_range)
