@@ -5,7 +5,7 @@
 #include <cstdlib>
 #include <new>
 
-#include "field.cuh"
+#include "field_simt_tile.cuh"
 
 namespace neddf {
 
@@ -31,15 +31,7 @@ struct PackArgs {
   int n_hidden;
 };
 
-// Hidden layers: channel c = cg + 16 i (cg = c % 16, i = c / 16) is stored at column
-// (i / 4) * 64 + cg * 4 + (i % 4), rows zero-padded up to k_pad.  Thread (s, cg) of the fp32
-// kernel owns channels {cg + 16 i}; its q-th float4 (i = 4q..4q+3) sits at q*64 + cg*4, so the
-// 16 lanes of a half-warp read 256 contiguous bytes per LDS.128 (no bank conflicts).
-__device__ __forceinline__ int simt_col(int c) {
-  int cg = c % 16, i = c / 16;
-  return (i / 4) * 64 + cg * 4 + (i % 4);
-}
-
+// Hidden layers: channel c at column simt_col(c), rows zero-padded up to k_pad.
 __global__ void pack_hidden_kernel(PackArgs a, float* __restrict__ w_dst, float* __restrict__ b_dst) {
   const int l = blockIdx.y;
   const int total = a.k_pad[l] * kWidth;

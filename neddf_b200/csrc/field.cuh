@@ -13,7 +13,7 @@ constexpr int kMaxEmbed = 16;        // max embed_pos_rank
 constexpr int kChunkRows = 16;       // weight rows per streamed chunk (fp32 engine)
 
 // One hidden layer as the kernels see it: its input is the concatenation of up to two
-// segments of the shared-memory "K space" (see field_simt.cu for the K-space map).
+// segments of the shared-memory "K space" (see field_simt_tile.cuh for the K-space map).
 struct LayerDesc {
   int k_in;        // reference input width (60, 256, 316, 343 ...)
   int k_pad;       // padded to a multiple of kChunkRows
@@ -89,6 +89,38 @@ __device__ __forceinline__ void field_map(const FieldParams& p, int64_t n, int64
     j = p.dists ? (int)(n % p.n_edges) : 0;
     out = n;
   }
+}
+
+// Network inputs of sample n: explicit samples, or the cone / point of its ray interval (ray.py:88-194 fused).
+// Samples at or past n_total get a fixed harmless input (their outputs are never written).
+struct SampleIn {
+  float pos[3], dir[3], var[3];
+};
+__device__ __forceinline__ SampleIn sample_input(const FieldParams& p, int64_t n, int64_t n_total) {
+  SampleIn r = {{0.f, 0.f, 0.f}, {0.f, 0.f, 1.f}, {0.f, 0.f, 0.f}};
+  if (n < n_total) {
+    if (p.dists) {
+      int64_t b, out;
+      int j;
+      field_map(p, n, b, j, out);
+      const float* row = p.dists + b * p.n_edges;
+      float o[3];
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        o[i] = p.ray_orig[3 * b + i];
+        r.dir[i] = p.ray_dir[3 * b + i];
+      }
+      sample_geometry(p.sampling_type, p.ray_radius, o, r.dir, row[j], far_edge(row, j, p.n_edges), r.pos, r.var);
+    } else {
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        r.pos[i] = p.pos[3 * n + i];
+        r.dir[i] = p.dir[3 * n + i];
+        r.var[i] = p.var[3 * n + i];
+      }
+    }
+  }
+  return r;
 }
 
 // Buffers of the training backward (all device, fp32, row-major)

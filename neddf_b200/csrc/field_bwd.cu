@@ -10,50 +10,15 @@
 //
 // Division of labour.  This kernel does the sample-local work: recompute post-activations from the
 // pre-activations the training forward saved, heads/penalty derivatives, activation backward
-// (needs f' and f''), and the data-gradient GEMMs  g_in = g_pre W^T  (same thread mapping and weight
-// streaming as the forward fp32 kernel, with transposed weights).  It writes, per layer, the
+// (needs f' and f''), and the data-gradient GEMMs  g_in = g_pre W^T  (the fp32 forward's tile skeleton,
+// field_simt_tile.cuh, with transposed weights).  It writes, per layer, the
 // post-activations and the pre-activation gradients; the weight gradients are then plain GEMMs over
 // all samples,  gW_l = X_l^T G_l  (+ bias = column sums), done by the host with cuBLAS
 // (torch.matmul) - a reduction over 10^5 samples is exactly what a library GEMM is for.
-#include "field_math.cuh"
-
-#include <algorithm>
+#include "field_simt_tile.cuh"
 
 namespace neddf {
 namespace bwd {
-
-constexpr int kTile = 16;
-constexpr int kPitch = 4 * kTile + 4;
-constexpr int kStages = 3;
-constexpr int kChunkFloats = kChunkRows * kWidth;
-constexpr int kThreads = 256;
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "BW_WAIT:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra BW_DONE;\n"
-      "bra BW_WAIT;\n"
-      "BW_DONE:\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
 
 // f, f', f'' with the reference's masks (tanh_exp.py:38-53; relu.py; leaky_relu.py)
 template <int ACT>
@@ -90,7 +55,7 @@ __device__ __forceinline__ float density_act_deriv(int act, float z) {
 }
 
 struct Scratch {  // per sample
-  float geo[9];
+  SampleIn in;
   float ddf[4], aux[4];  // head pre-activations: value (bias added) + 3 Jacobian entries
   HeadOut head;
   float gcolv[3];
@@ -185,29 +150,11 @@ __global__ void __launch_bounds__(kThreads, 1) field_backward_kernel(const __gri
   const int Lt = p.n_ddf - 1, Lc = n_hidden - 1;
 
   const int64_t n_tiles = (p.n + kTile - 1) / kTile;
-  int64_t my_tiles = 0;
-  if ((int64_t)blockIdx.x < n_tiles) my_tiles = (n_tiles - 1 - blockIdx.x) / gridDim.x + 1;
-  const int64_t total_chunks = my_tiles * P.chunks_per_tile;
-
-  if (tid == 0) {
-    for (int i = 0; i < kStages; ++i) mbar_init(&full[i], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
   for (int i = tid; i < kWidth * 2; i += kThreads) head_da[i] = p.w_head_da[i];
   for (int i = tid; i < kWidth * 4; i += kThreads) head_col[i] = p.w_head_col[i];
-  __syncthreads();
-  if (tid == 0) {
-    for (int g = 0; g < kStages && g < total_chunks; ++g) {
-      mbar_expect_tx(&full[g], kChunkFloats * 4);
-      bulk_g2s(wst + g * kChunkFloats, P.wt + (size_t)(g % P.chunks_per_tile) * kChunkFloats, kChunkFloats * 4,
-               &full[g]);
-    }
-  }
-  int64_t gchunk = 0;  // chunks consumed so far
-  int stage = 0;
-  uint32_t full_par = 0;
-  int cidx = 0;  // within-tile index of the next chunk to load
-  if (P.chunks_per_tile > 0) cidx = (int)((total_chunks < kStages ? total_chunks : (int64_t)kStages) % P.chunks_per_tile);
+  WeightRing ring{wst, full, P.wt, P.chunks_per_tile};
+  ring.init(n_tiles);
+  const LayerDesc gl = {kWidth, kWidth, {0, 0}, {kWidth, 0}, 0};  // the data-gradient GEMMs' input: all of gbuf
 
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const int64_t my_n = tile * kTile + s_slot;
@@ -249,43 +196,13 @@ __global__ void __launch_bounds__(kThreads, 1) field_backward_kernel(const __gri
         G[0][i] *= d1;
         G[1][i] *= d1;
         G[2][i] *= d1;
-        *reinterpret_cast<float4*>(&abuf[(size_t)(cg + 16 * i) * kPitch + 4 * s_slot]) =
-            make_float4(y, G[0][i], G[1][i], G[2][i]);
+        krow(abuf, cg + 16 * i, s_slot) = make_float4(y, G[0][i], G[1][i], G[2][i]);
       }
       store64(io.post, l, x, G);
     };
 
     // ---------------- geometry, embeddings (inputs of the weight-gradient GEMMs) -------------------
-    if (cg == 0) {
-      float pos[3] = {0.f, 0.f, 0.f}, dir[3] = {0.f, 0.f, 1.f}, var[3] = {0.f, 0.f, 0.f};
-      if (valid) {
-        if (p.dists) {
-          int64_t b = my_n / p.n_edges;
-          int j = (int)(my_n % p.n_edges);
-          const float* row = p.dists + b * p.n_edges;
-          float o[3];
-#pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            o[i] = p.ray_orig[3 * b + i];
-            dir[i] = p.ray_dir[3 * b + i];
-          }
-          sample_geometry(p.sampling_type, p.ray_radius, o, dir, row[j], far_edge(row, j, p.n_edges), pos, var);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            pos[i] = p.pos[3 * my_n + i];
-            dir[i] = p.dir[3 * my_n + i];
-            var[i] = p.var[3 * my_n + i];
-          }
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        sc.geo[i] = pos[i];
-        sc.geo[3 + i] = dir[i];
-        sc.geo[6 + i] = var[i];
-      }
-    }
+    if (cg == 0) sc.in = sample_input(p, my_n, p.n);
     __syncthreads();
     if (valid) {
       const int half = 3 * p.embed_pos;
@@ -293,23 +210,20 @@ __global__ void __launch_bounds__(kThreads, 1) field_backward_kernel(const __gri
       float* xes = io.xes + (size_t)my_n * 4 * p.n_e0;
       float* xcol = io.xcol + (size_t)my_n * 4 * koff;
       for (int idx = cg; idx < half; idx += 16) {
-        int e = idx / 3, d = idx - 3 * e;
-        PeEntry q = pe_entry(e, sc.geo[d], sc.geo[6 + d], p.lowpass[e]);
-        const float gs = q.freq * q.scale_s, g0 = q.freq * q.scale_0;
+        const PeRows r = pe_rows(p, sc.in, idx);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          const bool jr = (j == 1 + d);
-          xes[j * p.n_e0 + idx] = (j == 0) ? q.scale_s * q.s : (jr ? gs * q.c : 0.f);
-          xes[j * p.n_e0 + half + idx] = (j == 0) ? q.scale_s * q.c : (jr ? -gs * q.s : 0.f);
-          xcol[j * koff + idx] = (j == 0) ? q.scale_0 * q.s : (jr ? g0 * q.c : 0.f);
-          xcol[j * koff + half + idx] = (j == 0) ? q.scale_0 * q.c : (jr ? -g0 * q.s : 0.f);
+          xes[j * p.n_e0 + idx] = (&r.es_sin.x)[j];
+          xes[j * p.n_e0 + half + idx] = (&r.es_cos.x)[j];
+          xcol[j * koff + idx] = (&r.e0_sin.x)[j];
+          xcol[j * koff + half + idx] = (&r.e0_cos.x)[j];
         }
       }
       const int dhalf = 3 * p.embed_dir;
       for (int idx = cg; idx < dhalf; idx += 16) {
         int e = idx / 3, d = idx - 3 * e;
         float sn, cs;
-        sincosf((float)(1u << e) * sc.geo[3 + d], &sn, &cs);
+        sincosf((float)(1u << e) * sc.in.dir[d], &sn, &cs);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           xcol[j * koff + p.n_e0 + idx] = (j == 0) ? sn : 0.f;
@@ -322,25 +236,9 @@ __global__ void __launch_bounds__(kThreads, 1) field_backward_kernel(const __gri
     post_to_abuf(Lt);
     __syncthreads();
     {
-      float pd[4] = {0.f, 0.f, 0.f, 0.f}, pa[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 4
-      for (int kk = 0; kk < 16; ++kk) {
-        const int k = cg + 16 * kk;
-        const float4 a = *reinterpret_cast<const float4*>(&abuf[(size_t)k * kPitch + 4 * s_slot]);
-        const float2 w = *reinterpret_cast<const float2*>(&head_da[2 * k]);
-        pd[0] = fmaf(a.x, w.x, pd[0]); pd[1] = fmaf(a.y, w.x, pd[1]); pd[2] = fmaf(a.z, w.x, pd[2]); pd[3] = fmaf(a.w, w.x, pd[3]);
-        pa[0] = fmaf(a.x, w.y, pa[0]); pa[1] = fmaf(a.y, w.y, pa[1]); pa[2] = fmaf(a.z, w.y, pa[2]); pa[3] = fmaf(a.w, w.y, pa[3]);
-      }
-#pragma unroll
-      for (int m = 8; m > 0; m >>= 1)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          pd[j] += __shfl_xor_sync(0xffffffffu, pd[j], m);
-          pa[j] += __shfl_xor_sync(0xffffffffu, pa[j], m);
-        }
+      float pd[4], pa[4];
+      da_head(p, abuf, head_da, s_slot, cg, pd, pa);
       if (cg == 0) {
-        pd[0] += __ldg(p.b_head + 0);
-        pa[0] += __ldg(p.b_head + 1);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           sc.ddf[j] = pd[j];
@@ -363,35 +261,14 @@ __global__ void __launch_bounds__(kThreads, 1) field_backward_kernel(const __gri
     __syncthreads();
     {
       float pc[4][3];
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-#pragma unroll
-        for (int c = 0; c < 3; ++c) pc[j][c] = 0.f;
-#pragma unroll 4
-      for (int kk = 0; kk < 16; ++kk) {
-        const int k = cg + 16 * kk;
-        const float4 a = *reinterpret_cast<const float4*>(&abuf[(size_t)k * kPitch + 4 * s_slot]);
-        const float4 w = *reinterpret_cast<const float4*>(&head_col[4 * k]);
-        const float av[4] = {a.x, a.y, a.z, a.w};
-        const float wv[3] = {w.x, w.y, w.z};
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-#pragma unroll
-          for (int c = 0; c < 3; ++c) pc[j][c] = fmaf(av[j], wv[c], pc[j][c]);
-      }
-#pragma unroll
-      for (int m = 8; m > 0; m >>= 1)
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-#pragma unroll
-          for (int c = 0; c < 3; ++c) pc[j][c] += __shfl_xor_sync(0xffffffffu, pc[j][c], m);
+      col_head(p, abuf, head_col, s_slot, cg, pc);
       if (cg == 0) {
         const float gpen = (io.g_penalty && valid) ? io.g_penalty[nn] : 0.f;
         const float* pw = p.penalty_weight;
         float dotv[3];
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
-          const float col = pc[0][c] + __ldg(p.b_head + 2 + c);
+          const float col = pc[0][c];
           const float rc = fmaxf(-col, 0.f) + fmaxf(col - 1.0f, 0.f);
           const float gup = valid ? io.g_color[3 * nn + c] : 0.f;
           sc.gcolv[c] = gup + gpen * pw[4] * 2.0f * rc * ((col > 1.0f ? 1.0f : 0.0f) - (col < 0.0f ? 1.0f : 0.0f));
@@ -425,7 +302,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_backward_kernel(const __gri
       g.y = sc.gcolJ[0][0] * w.x + sc.gcolJ[0][1] * w.y + sc.gcolJ[0][2] * w.z;
       g.z = sc.gcolJ[1][0] * w.x + sc.gcolJ[1][1] * w.y + sc.gcolJ[1][2] * w.z;
       g.w = sc.gcolJ[2][0] * w.x + sc.gcolJ[2][1] * w.y + sc.gcolJ[2][2] * w.z;
-      *reinterpret_cast<float4*>(&gbuf[(size_t)k * kPitch + 4 * s_slot]) = g;
+      krow(gbuf, k, s_slot) = g;
     }
     // (every thread only touches its own (sample, channel) entries of gbuf until the next GEMM)
 
@@ -438,14 +315,14 @@ __global__ void __launch_bounds__(kThreads, 1) field_backward_kernel(const __gri
       for (int i = 0; i < 16; ++i) {
         float y, d1, d2;
         act_derivs<ACT>(x[i], y, d1, d2);
-        float* gp = &gbuf[(size_t)(cg + 16 * i) * kPitch + 4 * s_slot];
-        const float4 g = *reinterpret_cast<const float4*>(gp);
+        float4& g4 = krow(gbuf, cg + 16 * i, s_slot);
+        const float4 g = g4;
         // tanh_exp.py:84-85 : gx = gy f' + sum_i gG_i G_i f'' ; gG_i <- gG_i f'
         gx[i] = g.x * d1 + (g.y * G[0][i] + g.z * G[1][i] + g.w * G[2][i]) * d2;
         gG[0][i] = g.y * d1;
         gG[1][i] = g.z * d1;
         gG[2][i] = g.w * d1;
-        *reinterpret_cast<float4*>(gp) = make_float4(gx[i], gG[0][i], gG[1][i], gG[2][i]);
+        g4 = make_float4(gx[i], gG[0][i], gG[1][i], gG[2][i]);
         // post-activation of this layer = input of the next one (for the weight-gradient GEMMs)
         x[i] = y;
         G[0][i] *= d1;
@@ -458,49 +335,9 @@ __global__ void __launch_bounds__(kThreads, 1) field_backward_kernel(const __gri
       __syncthreads();
       // g_in[k] = sum_c gpre[c] W[k][c]  (linear.py:72-75): the forward GEMM loop with W^T chunks
       float acc[4][16];
+      ring_gemm(ring, gbuf, gl, s_slot, cg, acc);
 #pragma unroll
-      for (int j = 0; j < 4; ++j)
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[j][i] = 0.f;
-      for (int c = 0; c < kWidth / kChunkRows; ++c, ++gchunk) {
-        mbar_wait(&full[stage], full_par);
-        const float* wchunk = wst + stage * kChunkFloats + cg * 4;
-#pragma unroll 4
-        for (int rr = 0; rr < kChunkRows; ++rr) {
-          const int ks = c * kChunkRows + rr;
-          const float4 a = *reinterpret_cast<const float4*>(&gbuf[(size_t)ks * kPitch + 4 * s_slot]);
-          const float4* wp = reinterpret_cast<const float4*>(wchunk + rr * kWidth);
-          float w[16];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            float4 t = wp[q * 16];
-            w[4 * q + 0] = t.x; w[4 * q + 1] = t.y; w[4 * q + 2] = t.z; w[4 * q + 3] = t.w;
-          }
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            acc[0][i] = fmaf(a.x, w[i], acc[0][i]);
-            acc[1][i] = fmaf(a.y, w[i], acc[1][i]);
-            acc[2][i] = fmaf(a.z, w[i], acc[2][i]);
-            acc[3][i] = fmaf(a.w, w[i], acc[3][i]);
-          }
-        }
-        __syncthreads();
-        if (tid == 0 && gchunk + kStages < total_chunks) {
-          mbar_expect_tx(&full[stage], kChunkFloats * 4);
-          bulk_g2s(wst + stage * kChunkFloats, P.wt + (size_t)cidx * kChunkFloats, kChunkFloats * 4, &full[stage]);
-        }
-        if (gchunk + kStages < total_chunks) {
-          if (++cidx == P.chunks_per_tile) cidx = 0;
-        }
-        if (++stage == kStages) {
-          stage = 0;
-          full_par ^= 1;
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        *reinterpret_cast<float4*>(&gbuf[(size_t)(cg + 16 * i) * kPitch + 4 * s_slot]) =
-            make_float4(acc[0][i], acc[1][i], acc[2][i], acc[3][i]);
+      for (int i = 0; i < 16; ++i) krow(gbuf, cg + 16 * i, s_slot) = make_float4(acc[0][i], acc[1][i], acc[2][i], acc[3][i]);
     };
 
     // colour layers, last to first (the h part of colour layer 0's input is the trunk output)
@@ -525,13 +362,11 @@ __global__ void __launch_bounds__(kThreads, 1) field_backward_kernel(const __gri
     for (int i = 0; i < 16; ++i) {
       const int k = cg + 16 * i;
       const float2 w = *reinterpret_cast<const float2*>(&head_da[2 * k]);
-      float* gp = &gbuf[(size_t)k * kPitch + 4 * s_slot];
-      float4 g = *reinterpret_cast<const float4*>(gp);
+      float4& g = krow(gbuf, k, s_slot);
       g.x += sc.gddf[0] * w.x + sc.gaux[0] * w.y;
       g.y += sc.gddf[1] * w.x + sc.gaux[1] * w.y;
       g.z += sc.gddf[2] * w.x + sc.gaux[2] * w.y;
       g.w += sc.gddf[3] * w.x + sc.gaux[3] * w.y;
-      *reinterpret_cast<float4*>(gp) = g;
     }
 
     // distance trunk, last to first (layer 0's input is the embedding: no data gradient needed)
@@ -553,10 +388,6 @@ struct PackT {
   int order[kMaxHidden];   // order[i] = layer processed i-th
   int n;
 };
-__device__ __forceinline__ int simt_col(int c) {
-  int cg = c % 16, i = c / 16;
-  return (i / 4) * 64 + cg * 4 + (i % 4);
-}
 __global__ void pack_wt_kernel(PackT a, float* __restrict__ dst) {
   const int slot = blockIdx.y;
   const int l = a.order[slot];
@@ -598,20 +429,8 @@ int32_t launch_field_backward(const neddf_field* f, FieldParams& p, const Backwa
   P.chunks_per_tile = f->wt_chunks;
   size_t smem = bwd::smem_bytes();
   if (smem > 227 * 1024) return fail(NEDDF_E_UNSUPPORTED, "field backward: shared memory budget exceeded");
-  int64_t n_tiles = (p.n + bwd::kTile - 1) / bwd::kTile;
-  int grid = (int)std::min<int64_t>(n_tiles, sm_count());
-  auto launch = [&](auto kern) -> int32_t {
-    NEDDF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<grid, bwd::kThreads, smem, s>>>(P);
-    NEDDF_LAUNCH_CHECK();
-    return NEDDF_OK;
-  };
-  switch (p.hidden_act) {
-    case NEDDF_ACT_TANHEXP: return launch(bwd::field_backward_kernel<NEDDF_ACT_TANHEXP>);
-    case NEDDF_ACT_RELU: return launch(bwd::field_backward_kernel<NEDDF_ACT_RELU>);
-    case NEDDF_ACT_LEAKYRELU: return launch(bwd::field_backward_kernel<NEDDF_ACT_LEAKYRELU>);
-  }
-  return fail(NEDDF_E_INVALID, "field backward: unknown activation");
+  return launch_tiles(bwd::field_backward_kernel<NEDDF_ACT_TANHEXP>, bwd::field_backward_kernel<NEDDF_ACT_RELU>,
+                      bwd::field_backward_kernel<NEDDF_ACT_LEAKYRELU>, p.hidden_act, P, p.n, smem, "field backward", s);
 }
 
 }  // namespace neddf

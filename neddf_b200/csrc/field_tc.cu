@@ -143,35 +143,12 @@ __device__ __forceinline__ void tma_bulk_g2s_pair(uint32_t dst_smem, const void*
 // ---------------------------------------------------------------------------------------------
 // geometry of the tile's samples -> scratch (one thread per sample)
 __device__ __forceinline__ void tile_geometry(const FieldParams& p, float (*geo)[12], int64_t n0, int s, int64_t n_total) {
-  float pos[3] = {0.f, 0.f, 0.f}, dir[3] = {0.f, 0.f, 1.f}, var[3] = {0.f, 0.f, 0.f};
-  const int64_t n = n0 + s;
-  if (n < n_total) {
-    if (p.dists) {
-      int64_t b, out;
-      int j;
-      field_map(p, n, b, j, out);
-      const float* row = p.dists + b * p.n_edges;
-      float o[3];
-#pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        o[i] = p.ray_orig[3 * b + i];
-        dir[i] = p.ray_dir[3 * b + i];
-      }
-      sample_geometry(p.sampling_type, p.ray_radius, o, dir, row[j], far_edge(row, j, p.n_edges), pos, var);
-    } else {
-#pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        pos[i] = p.pos[3 * n + i];
-        dir[i] = p.dir[3 * n + i];
-        var[i] = p.var[3 * n + i];
-      }
-    }
-  }
+  const SampleIn in = sample_input(p, n0 + s, n_total);
 #pragma unroll
   for (int i = 0; i < 3; ++i) {
-    geo[s][i] = pos[i];
-    geo[s][3 + i] = dir[i];
-    geo[s][6 + i] = var[i];
+    geo[s][i] = in.pos[i];
+    geo[s][3 + i] = in.dir[i];
+    geo[s][6 + i] = in.var[i];
   }
 }
 
@@ -283,7 +260,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
       mbar_init(&sc->full[i], 1);
       mbar_init(&sc->empty[i], PAIR ? 2 * kConsumerWarps : kConsumerWarps);
     }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_fence_init();
   }
   __syncthreads();
   if (PAIR) cluster_sync_all();  // the partner's barriers exist before any multicast or remote arrival

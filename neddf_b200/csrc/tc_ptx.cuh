@@ -1,8 +1,9 @@
-// Hopper (sm_90a) building blocks of the tensor-core kernels (field_tc.cu, wgrad.cu): wgmma / mbarrier /
-// TMA bulk-copy wrappers, operand layouts and the split-fp16 helpers.
+// Hopper (sm_90a) building blocks of the tensor-core kernels (field_tc.cu, wgrad.cu): wgmma wrappers, operand
+// layouts and the split-fp16 helpers, on top of the mbarrier / TMA bulk-copy wrappers of mbarrier.cuh.
 #pragma once
 
 #include "field_math.cuh"
+#include "mbarrier.cuh"
 
 #include <cuda_fp16.h>
 
@@ -30,40 +31,9 @@ __host__ __device__ __forceinline__ uint32_t wchunk_off(int m, int k) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// PTX wrappers
+// PTX wrappers (the mbarrier and bulk-copy ones are in mbarrier.cuh)
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "TC_WAIT:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra TC_DONE;\n"
-      "bra TC_WAIT;\n"
-      "TC_DONE:\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// TMA 1-D bulk copy global -> shared memory, completion counted in bytes on an mbarrier
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tma_bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem),
-               "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
 
 // wgmma shared-memory matrix descriptor, no swizzle: start, leading (K-direction) and stride (M/N-direction)
 // byte offsets between core matrices
