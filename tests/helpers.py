@@ -41,6 +41,29 @@ def assert_parity(new, ref, tol, kinked=False, what=""):
     assert n_out <= max(2, int(1e-2 * err.size)) and float(err.max()) < 5e-2, (what, n_out, err.size, float(err.max()))
 
 
+def check_neus_normal(P64, nc, pos, got, ref, what):
+    """A NeuS normal (or the colour, which reads it) [B,S,3] against its reference at the parity bound.  With ReLU the
+    normal is piecewise constant in the hidden units' signs: a sample whose fp64 pre-activation lies within fp32 rounding
+    of zero may land on the other side in a differently ordered fp32 sum, and its normal then differs by one unit's
+    contribution.  Such samples - and only such samples - are exempt: every outlier must show that witness
+    (orc.neus_kink_distance under the fp64 parameters ``P64``), and there may be few
+    (tests/test_neus_oracle.py::test_relu_normal_outliers_sit_on_kinks shows the reference restatement doing the same
+    under a one-ulp shift of its inputs).  Returns the largest error."""
+    err = np.abs(got - ref).max(axis=-1) / max(float(np.abs(ref).max()), 1e-30)
+    assert err.shape == pos.shape[:2]
+    bad = np.argwhere(err >= PARITY_TOL)
+    if nc.activation_type != "ReLU":
+        assert len(bad) == 0, (what, float(err.max()))
+        return float(err.max())
+    kink = orc.neus_kink_distance(P64, nc, pos.double()).numpy()
+    report = [(tuple(int(v) for v in i), float(err[tuple(i)]), float(kink[tuple(i)])) for i in bad]
+    assert len(bad) <= max(2, err.size // 500) and float(err.max()) < 5e-2, (what, report)
+    assert all(k < 5e-6 for _, _, k in report), (what, "outlier away from every ReLU kink", report)
+    if report:
+        print(f"[neus normal] {what}: {len(report)} of {err.size} samples on a ReLU kink: {report}")
+    return float(err.max())
+
+
 class Case:
     """One golden case: configs, weights, camera, inputs and the reference's outputs."""
 

@@ -3,12 +3,10 @@
 NeRF variant, training backward on the GPU (csrc/nerf_train.cu + neddf_wgrad behind neddf_b200.NeRF with
 training_kernels=True) against the REAL reference's autograd gradients (tests/golden/make_nerf_train_golden.py).
 
-STATUS - read before trusting a green or red mark here: this kernel was written after the round's GPU budget was
-spent.  Its tile program is validated on the CPU (tests/test_nerf_train_emul.py: 256 OS threads per CTA, the same
-fixtures, AddressSanitizer / UBSan / ThreadSanitizer, the autograd glue over a fake library), but these tests have never
-run on hardware.  They are therefore NON-STRICT expected failures: an XPASS in the driver's log is the first hardware
-run succeeding, an XFAIL is a finding for the next round; neither hides behind the rest of the suite, and the feature
-stays opt-in (NeRF.training_kernels) either way."""
+Status: the tile program is also validated on the CPU (tests/test_nerf_train_emul.py: 256 OS threads per CTA, the same
+fixtures, AddressSanitizer / UBSan / ThreadSanitizer, the autograd glue over a fake library).  On the H100 these checks
+pass since the per-column power-of-two operand scaling of neddf_wgrad, and they are ordinary tests: a red mark here is
+a regression.  The feature stays opt-in (NeRF.training_kernels)."""
 import sys
 
 import numpy as np

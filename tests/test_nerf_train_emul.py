@@ -8,8 +8,8 @@ the upstream gradients (d loss / d density,
 d loss / d colour per sample, captured with tensor hooks) of fixtures recorded from the REAL reference's autograd
 (tests/golden/make_nerf_train_golden.py).  The parameter gradients are then assembled exactly as the GPU path does -
 gW = X^T G over all samples, bias = column sums - with numpy standing in for neddf_wgrad, and compared with the
-reference's.  STATUS of the kernel itself: not yet run on hardware (the round's GPU budget was spent when it was
-written); tests/test_nerf_train_gpu.py holds the GPU tests."""
+reference's.  The compiled kernel is tested on the GPU by tests/test_zzz_nerf_train_gpu.py (the same fixtures) and
+tests/test_nerf_neus_configs_gpu.py (the structures of tests/nerf_neus_configs.py)."""
 import ctypes as C
 import json
 import os
@@ -21,6 +21,7 @@ import pytest
 import torch
 
 from oracle import neddf_oracle as orc
+from tests import nerf_neus_configs as ncfg
 from tests.helpers import GOLDEN, PARITY_TOL, assert_parity, nerr
 from tests.test_nerf_oracle import NerfCase
 
@@ -313,6 +314,35 @@ def test_emulated_backward_leaky_density_and_ragged_tiles(emul):
             ref = Pg[k].grad.numpy()
             ref = ref.T if k.endswith(".weight") else ref  # the oracle keeps [in,out]
             assert nerr(v, ref) < 2e-5, (B, S, k, nerr(v, ref))
+
+
+@pytest.mark.parametrize("name", ["N2_max_embed", "N4_deep_train"])  # about 2 s each on the CPU
+def test_emulated_kernels_at_table_structures(emul, name):
+    """Structures of tests/nerf_neus_configs.py on the CPU: 60 + 30 embedding rows with a skip after layer 0 (N2), the
+    training backward's 12 layers with consecutive skips (N4).  Forward on 65 explicit samples against the oracle,
+    backward on 5 x 13 cone samples against fp64 autograd."""
+    nc, alpha = ncfg.config(name), ncfg.lowpass_alpha(name)
+    names = [n for n, _, _ in ncfg.layer_shapes(name)]
+    sd = ncfg.state_dict(name)
+    ws = [np.ascontiguousarray(sd[n + ".weight"].numpy()) for n in names]
+    bs = [np.ascontiguousarray(sd[n + ".bias"].numpy()) for n in names]
+    P = ncfg.params(name)
+    pos, dd, var = ncfg.samples(1, 65, ncfg.SEED[name] + 1)
+    dens, col = run_forward(emul, nc, alpha, ws, bs, samples=(pos, dd, var), nblocks=2)
+    with torch.no_grad():
+        ref = orc.nerf_forward({k: v.double() for k, v in P.items()}, nc, alpha, pos.double(), dd.double(), var.double())
+    for k, v in (("density", dens), ("color", col)):
+        assert nerr(v, ref[k].numpy().reshape(v.shape)) < PARITY_TOL, k
+    d, o, dists = ncfg.rays(5, 13, ncfg.SEED[name] + 2)
+    gd, gc, _ = ncfg.upstream(5, 13, ncfg.SEED[name] + 3)
+    Pg = {k: v.double().requires_grad_(True) for k, v in P.items()}
+    out = orc.nerf_forward(Pg, nc, alpha, *(t.double() for t in orc.cone_samples(d, o, dists, orc.CONE_RAY_RADIUS)))
+    ((out["density"] * gd.double()).sum() + (out["color"] * gc.double()).sum()).backward()
+    buf, gdn, gcn = run_backward(emul, nc, alpha, ws, bs, d, o, dists, "cone", gd.numpy(), gc.numpy())
+    for k, v in assemble_grads(nc, names, buf, gdn, gcn).items():
+        ref = Pg[k].grad.numpy()
+        ref = ref.T if k.endswith(".weight") else ref
+        assert nerr(v, ref) < 2e-5, (k, nerr(v, ref))
 
 
 class _FakeLib:

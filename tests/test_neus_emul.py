@@ -15,6 +15,7 @@ import pytest
 import torch
 
 from oracle import neddf_oracle as orc
+from tests import nerf_neus_configs as ncfg
 from tests.helpers import PARITY_TOL, nerr
 from tests.test_neus_oracle import NeusCase
 
@@ -140,7 +141,16 @@ class _Synthetic:
 def test_emulated_kernel_layer_table_extremes(emul, kw):
     """Configurations at the edges of what neddf_neus_create accepts, against the oracle (70 samples: one full tile
     and a ragged one whose last SDF sub-tile is partly empty)."""
-    c = _Synthetic(orc.NeusConfig(**kw), seed=5)
+    _check_against_oracle(emul, _Synthetic(orc.NeusConfig(**kw), seed=5))
+
+
+@pytest.mark.parametrize("name", ["S1_one_sdf", "S3_deepest"])  # about 3.5 s each on the CPU
+def test_emulated_kernel_at_table_structures(emul, name):
+    """Structures of tests/nerf_neus_configs.py: the sdf from the first layer, both trunks 12 deep."""
+    _check_against_oracle(emul, _Synthetic(ncfg.config(name), seed=ncfg.SEED[name]))
+
+
+def _check_against_oracle(emul, c):
     g = torch.Generator().manual_seed(9)
     pos = torch.rand(1, 70, 3, generator=g) * 2 - 1
     dd = torch.nn.functional.normalize(torch.randn(1, 70, 3, generator=g), dim=-1)

@@ -8,7 +8,7 @@ import pytest
 import torch
 
 from oracle import neddf_oracle as orc
-from tests.helpers import PARITY_TOL, nerr
+from tests.helpers import PARITY_TOL, check_neus_normal, nerr
 from tests.test_neus_oracle import NeusCase
 
 pytestmark = pytest.mark.gpu
@@ -34,24 +34,7 @@ def build(c: NeusCase):
 
 
 def check_normal(c: NeusCase, tag: str, pos, got, ref, what):
-    """The normal (and the colour, which reads it) against the reference at the parity bound.  With ReLU the normal is piecewise
-    constant in the hidden units' signs: a sample whose fp64 pre-activation lies within fp32 rounding of zero may
-    land on the other side in a differently ordered fp32 sum, and its normal then differs by one unit's contribution.
-    Such samples - and only such samples - are exempt: every outlier must show that witness, and there may be few
-    (tests/test_neus_oracle.py::test_relu_normal_outliers_sit_on_kinks shows the reference restatement doing the same
-    under a one-ulp shift of its inputs)."""
-    err = np.abs(got - ref).max(axis=-1) / np.abs(ref).max()
-    assert err.shape == pos.shape[:2]
-    bad = np.argwhere(err >= PARITY_TOL)
-    if c.nc.activation_type != "ReLU":
-        assert len(bad) == 0, (tag, what, float(err.max()))
-        return
-    kink = orc.neus_kink_distance(c.params(tag, torch.float64), c.nc, pos.double()).numpy()
-    report = [(tuple(int(v) for v in i), float(err[tuple(i)]), float(kink[tuple(i)])) for i in bad]
-    assert len(bad) <= max(2, err.size // 500) and float(err.max()) < 5e-2, (tag, what, report)
-    assert all(k < 5e-6 for _, _, k in report), (tag, what, "outlier away from every ReLU kink", report)
-    if report:
-        print(f"[neus normal] {tag} / {what}: {len(report)} of {err.size} samples on a ReLU kink: {report}")
+    check_neus_normal(c.params(tag, torch.float64), c.nc, pos, got, ref, f"{tag} / {what}")
 
 
 @pytest.mark.parametrize("name", ["relu", "tanhexp"])

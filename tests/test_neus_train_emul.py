@@ -20,6 +20,7 @@ import pytest
 import torch
 
 from oracle import neddf_oracle as orc
+from tests import nerf_neus_configs as ncfg
 from tests import neus_train_oracle as nto
 from tests.helpers import GOLDEN, assert_parity, nerr
 
@@ -296,6 +297,35 @@ def test_emulated_backward_optional_gradients_and_ragged_tiles(emul):
             ref = P[k].grad.numpy()
             ref = ref.T if k.endswith(".weight") else ref
             assert nerr(v, ref) < 2e-5, (n, k, nerr(v, ref))
+
+
+@pytest.mark.parametrize("name", ["S1_one_sdf", "S3_deepest"])  # 0.2 s and 6.5 s on the CPU
+def test_emulated_backward_at_table_structures(emul, name):
+    """Structures of tests/nerf_neus_configs.py: the sdf from the first layer (ReLU: the kinked rule of
+    helpers.assert_parity), both trunks 12 deep (tanhExp); 65 samples with upstream gradients on all four outputs,
+    against fp64 autograd through the restatement."""
+    nc = ncfg.config(name)
+    names = [n for n, _, _ in ncfg.layer_shapes(name)]
+    sd = ncfg.state_dict(name)
+    ws = [np.ascontiguousarray(sd[n + ".weight"].numpy()) for n in names]
+    bs = [np.ascontiguousarray(sd[n + ".bias"].numpy()) for n in names]
+    var = sd["variance"].numpy().reshape(1)
+    pos, dd, _ = ncfg.samples(1, 65, ncfg.SEED[name] + 1)
+    g = torch.Generator().manual_seed(ncfg.SEED[name])
+    gs, gd, gc, gn = (torch.randn(1, 65, generator=g), torch.randn(1, 65, generator=g), torch.randn(1, 65, 3, generator=g),
+                      torch.randn(1, 65, 3, generator=g))
+    P = nto.params_from_torch(ws, bs, names, var, torch.float64)
+    out = nto.neus_train_forward_jac(P, nc, pos.double(), dd.double())
+    ((out["sdf"] * gs.double()).sum() + (out["density"] * gd.double()).sum() + (out["color"] * gc.double()).sum()
+     + (out["normal"] * gn.double()).sum()).backward()
+    buf, gcn = run_backward(emul, nc, ws, bs, var, gd.numpy(), gc.numpy(), samples=(pos, dd), g_sdf=gs.numpy(), g_normal=gn.numpy())
+    for k, v in assemble_grads(nc, names, buf, gcn).items():
+        ref = P[k].grad.numpy()
+        ref = ref.T if k.endswith(".weight") else ref
+        if nc.activation_type == "ReLU" and np.ndim(v) > 0:
+            assert_parity(v, ref, 1e-4, kinked=True, what=k)
+        else:
+            assert nerr(v, ref) < 2e-5, (k, nerr(v, ref))
 
 
 class _FakeLib:

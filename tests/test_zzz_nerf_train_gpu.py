@@ -1,15 +1,14 @@
-"""NeRF variant, training backward on the GPU: first hardware run of csrc/nerf_train.cu (see tests/nerf_train_gpu_child.py
-for the checks and their status).  Each check runs in a CHILD PROCESS with a timeout and this file is collected last:
-a fault or a hang of a kernel that has never run on hardware cannot poison the CUDA context of the validated suite.
-NON-STRICT expected failures: XPASS = the first hardware run succeeded, XFAIL = a finding for the next round."""
+"""NeRF variant, training backward on the GPU: csrc/nerf_train.cu against the real reference's autograd gradients (see
+tests/nerf_train_gpu_child.py for the checks).  Each check runs in a CHILD PROCESS with a timeout and this file is
+collected last, so that a fault or a hang of the opt-in kernel cannot poison the CUDA context of the rest of the suite;
+a failing check fails the suite.  tests/test_nerf_neus_configs_gpu.py holds the same backward at other structures."""
 import os
 import subprocess
 import sys
 
 import pytest
 
-pytestmark = [pytest.mark.gpu,
-              pytest.mark.xfail(strict=False, reason="first hardware run of csrc/nerf_train.cu (validated by host emulation only)")]
+pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
