@@ -85,6 +85,17 @@ def _camera_host(camera) -> Tuple[Any, Any, Any]:
     return out
 
 
+# neddf_composite_backward keeps T and o of all intervals of its 8 rays in shared memory, 8 * 2 * 4 B per interval,
+# and refuses more than 200 KB (csrc/composite.cu): at most 3201 edges per ray can be trained through.
+COMPOSITE_BACKWARD_MAX_EDGES = 200 * 1024 // (8 * 2 * 4) + 1
+
+
+def _check_trainable_edges(n_edges: int) -> None:
+    if n_edges > COMPOSITE_BACKWARD_MAX_EDGES:
+        raise RuntimeError(f"neddf_b200: {n_edges} edges per ray are more than the compositing training backward "
+                           f"takes ({COMPOSITE_BACKWARD_MAX_EDGES}); render without gradients or with fewer samples")
+
+
 class _CompositeFn(torch.autograd.Function):
     """Differentiable compositing: forward neddf_composite, backward neddf_composite_backward
     (gradients w.r.t. densities, colours and penalties; edge distances carry none, like the
@@ -93,6 +104,7 @@ class _CompositeFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, dists, densities, colors, penalties, max_dist, status):
         B, E = dists.shape
+        _check_trainable_edges(E)
         device = dists.device
         weight = torch.empty(B, E - 1, device=device, dtype=torch.float32)
         depth = torch.empty(B, device=device, dtype=torch.float32)
@@ -412,6 +424,8 @@ class NeRFRender(BaseNeuralRender):
         uv = uv.contiguous()
         B = uv.shape[0]
         device = uv.device
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            _check_trainable_edges(self.sample_coarse + self.sample_fine + 2)  # before the forward, not after it
         hR, hT, hC = _camera_host(camera)
         with torch.cuda.device(device):
             ray_dir = torch.empty(B, 3, device=device, dtype=torch.float32)

@@ -492,7 +492,7 @@ def pdf_cdf(weights: Tensor, smooth: bool = False) -> Tensor:
     """Sanitise, +1e-2, [neighbour-max smoothing when not cat_coarse, :61-68], L1-normalise, cumsum with
     leading 0 (base_neural_render.py:52-72)."""
     w = sanitise_weights(weights) + 1e-2
-    if smooth:
+    if smooth and w.shape[-1] > 1:  # the reference writes weights[:, 1:-1], which is empty for one interval
         w1 = torch.maximum(w[:, 2:], w[:, 1:-1])
         w2 = torch.maximum(w[:, :-2], w[:, 1:-1])
         w = torch.cat([w[:, :1], 0.5 * (w1 + w2), w[:, -1:]], -1)
