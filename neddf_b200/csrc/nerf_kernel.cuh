@@ -300,11 +300,29 @@ inline size_t build_program(const neddf_nerf_config_t* c, Params& P, bool transp
   return off;
 }
 
+// torch's tensors in the order of layer_shapes
+using Tensors = simt::Linears<kMaxLayers + 3>;
+
+// Packs t into the buffer laid out by build_program (work items t0, t0 + stride, ... as simt::pack_linear): hidden
+// layers 0..L-1 are tensors 0..L-1, the colour branch's first layer (layer L) is tensor L + 1, each with its transposed
+// pack if build_program reserved one; then the small heads as stored by torch: density [256] + bias (tensor L), colour
+// [3][128] + 3 biases (tensor L + 2).
+__device__ __forceinline__ void pack(int t0, int stride, const Params& P, const Tensors& t, float* dst) {
+  const int L = P.n_layers;
+  for (int l = 0; l <= L; ++l) {
+    const int i = (l < L) ? l : L + 1;
+    const Layer& ly = P.layer[l];
+    simt::pack_linear(t0, stride, t.w[i], t.b[i], t.n_in[i], t.n_out[i], ly.k_pad, ly.kt_pad, 0, dst + ly.w_off, dst + ly.b_off,
+                      dst + ly.wt_off);
+  }
+  for (int i = t0; i < kW; i += stride) dst[P.w_density_off + i] = t.w[L][i];
+  if (t0 == 0) dst[P.w_density_off + kW] = t.b[L][0];
+  for (int i = t0; i < 3 * (kW / 2); i += stride) dst[P.w_col2_off + i] = t.w[L + 2][i];
+  for (int i = t0; i < 3; i += stride) dst[P.w_col2_off + 3 * (kW / 2) + i] = t.b[L + 2][i];
+}
+
 #ifdef __CUDACC__
-// Packs torch's tensors (the order of layer_shapes) into the buffer laid out by build_program (nerf_simt.cu): the
-// set_weights of both NeRF handles.
-int32_t pack_weights(const Params& P, const int* shape_in, const int* shape_out, const float* const* d_w, const float* const* d_b,
-                     float* dst, cudaStream_t s);
+__global__ void nerf_pack_kernel(const __grid_constant__ Params P, const __grid_constant__ Tensors t, float* dst);  // nerf_simt.cu
 #endif
 
 }  // namespace nerf

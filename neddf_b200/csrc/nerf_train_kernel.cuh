@@ -57,10 +57,6 @@ inline const char* unsupported(const neddf_nerf_config_t* c) {
 // fills the network part of P with the transposed packs; returns the floats of the packed weight buffer
 inline size_t build_program(const neddf_nerf_config_t* c, Params& P) { return nerf::build_program(c, P, /*transposed=*/true); }
 
-// entries (k, c) of a layer's forward and transposed packs (simt::pack_linear): the host emulation's packing
-__device__ __forceinline__ float pack_fwd(const float* w, int n_in, int n_out, int k, int c) { return simt::pack_entry(w, n_in, n_out, k, c); }
-__device__ __forceinline__ float pack_bwd(const float* w, int n_in, int n_out, int k, int c) { return simt::pack_t(w, n_in, n_out, 0, k, c); }
-
 // shared memory: the forward's map, then the per-sample upstream gradients
 constexpr int kOffUp = nerf::kSmemFloats;  // [kT][4] g_color (3), g_zd
 constexpr int kSmemFloats = kOffUp + kT * 4;

@@ -40,7 +40,6 @@ using simt::kChunk;
 using simt::kT;
 using simt::kThreads;
 using simt::kW;
-using simt::pack_entry;
 constexpr int kSub = 16;     // samples per SDF sub-tile (4 columns each)
 constexpr int kMaxE = 64;    // rows reserved for the position embedding (6 * rank <= 64)
 constexpr int kMaxX = 32;    // colour input head [pos 3 | dir embedding 6 * rank | normal 3] (<= 32 rows)
@@ -91,21 +90,27 @@ constexpr int kOffSdf = kOffGeo + kT * 6;         // [kT] sdf of the tile's samp
 constexpr int kSmemFloats = kOffSdf + kT;
 constexpr size_t kSmemBytes = (size_t)kSmemFloats * sizeof(float);
 
-// Activation with first derivative.  ReLU: torch.relu and its autograd slope (x > 0); tanhExp: nn_module/tanh_exp.py
-// :26-31 forward, :57-60 backward (d = tx - x ex (tx^2 - 1), 1 above the threshold).
-__device__ __forceinline__ void act_fd(int act, float x, float& y, float& d1) {
+// Activation with its slope d1 and the reference's second derivative d2 (the training backward's; the forward
+// ignores d2).  ReLU: torch.relu and its autograd slope (x > 0), d2 = 0.  tanhExp: nn_module/tanh_exp.py :26-31
+// forward, :57-60 backward (d1 = tx - x ex (tx^2 - 1), 1 above the threshold); it saves ex = exp(x), tx = tanh(ex)
+// without a graph, so double backward differentiates d1 through the explicit x only: d2 = ex (1 - tx^2) (0 above the
+// threshold), not the true second derivative.
+__device__ __forceinline__ void act_fdd(int act, float x, float& y, float& d1, float& d2) {
   if (act == NEDDF_ACT_TANHEXP) {
     const float ex = expf(x);
     const float tx = tanhf(ex);
     y = x * tx;
     d1 = tx - x * ex * (tx * tx - 1.0f);
+    d2 = ex * (1.0f - tx * tx);
     if (x > 20.0f) {
       y = x;
       d1 = 1.0f;
+      d2 = 0.0f;
     }
   } else {
     d1 = (x > 0.0f) ? 1.0f : 0.0f;
     y = (x > 0.0f) ? x : 0.0f;
+    d2 = 0.0f;
   }
 }
 
@@ -129,116 +134,143 @@ __device__ __forceinline__ void layer_gemm(Ctx& cx, const Params& P, const Layer
   simt::gemm(cx, P.w + L.w_off, L.k_pad, A, L.n_a, B, L.n_b, smem + kOffW, acc);
 }
 
+// Geometry of tile n0's samples (one thread per sample) into geo and rows 0..2 of X (position, neus.py:145), then the
+// direction embedding into X (neus.py:120, four threads per sample).  Exit: NOT behind a barrier - X is first read by
+// the colour trunk, behind the barriers of the SDF trunk.
+template <class Ctx>
+__device__ __forceinline__ void prologue(Ctx& cx, const Params& P, float* smem, int64_t n0) {
+  float* X = smem + kOffX;
+  float* geo = smem + kOffGeo;
+  const int tid = cx.tid;
+  if (tid < kT) {
+    float pos[3] = {0.f, 0.f, 0.f}, dir[3] = {0.f, 0.f, 1.f}, var[3];
+    const int64_t n = n0 + tid;
+    if (n < P.n) {
+      if (P.dists) {
+        const int64_t b = n / P.n_edges;
+        const int j = (int)(n - b * P.n_edges);
+        const float* row = P.dists + b * P.n_edges;
+        float o[3];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+          o[i] = P.ray_orig[3 * b + i];
+          dir[i] = P.ray_dir[3 * b + i];
+        }
+        sample_geometry(P.sampling_type, P.ray_radius, o, dir, row[j], far_edge(row, j, P.n_edges), pos, var);
+      } else {
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+          pos[i] = P.pos[3 * n + i];
+          dir[i] = P.dir[3 * n + i];
+        }
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+      geo[tid * 6 + i] = pos[i];
+      geo[tid * 6 + 3 + i] = dir[i];
+      X[i * kT + tid] = pos[i];
+    }
+  }
+  cx.sync();
+  const int dhalf = 3 * P.embed_dir;
+  const int s = tid >> 2, sub4 = tid & 3;
+  for (int idx = sub4; idx < dhalf; idx += 4) {
+    const int e = idx / 3, d = idx - 3 * e;
+    float sn, cs;
+    sincosf((float)(1u << e) * geo[s * 6 + 3 + d], &sn, &cs);
+    X[(3 + idx) * kT + s] = sn;
+    X[(3 + dhalf + idx) * kT + s] = cs;
+  }
+}
+
+// Position embedding with its Jacobian (neus.py:119) of SDF sub-tile `sub` into E (sixteen threads per sample; column
+// 4 s + r: value, d/dx, d/dy, d/dz of sample s).  Exit: behind a barrier.
+template <class Ctx>
+__device__ __forceinline__ void sdf_embedding(Ctx& cx, const Params& P, float* smem, int sub) {
+  float* E = smem + kOffE;
+  const int ehalf = 3 * P.embed_pos;  // rows of the sine block
+  const int s = cx.tid >> 4, lane16 = cx.tid & 15;
+  const float* p3 = smem + kOffGeo + (kSub * sub + s) * 6;
+  for (int idx = lane16; idx < ehalf; idx += 16) {
+    const int e = idx / 3, d = idx - 3 * e;
+    const float f = (float)(1u << e);
+    float sn, cs;
+    sincosf(f * p3[d], &sn, &cs);
+    float4 vs = make_float4(sn, 0.f, 0.f, 0.f), vc = make_float4(cs, 0.f, 0.f, 0.f);
+    const float js = f * cs, jc = -(f * sn);
+    if (d == 0) { vs.y = js; vc.y = jc; }
+    else if (d == 1) { vs.z = js; vc.z = jc; }
+    else { vs.w = js; vc.w = jc; }
+    *reinterpret_cast<float4*>(E + idx * kT + 4 * s) = vs;
+    *reinterpret_cast<float4*>(E + (ehalf + idx) * kT + 4 * s) = vc;
+  }
+  cx.sync();
+}
+
+// SDF layer epilogue of channel ch for the sample in column `col` of the colour trunk (sub-tile column sg): returns
+// (y, J_y) = (f(z), f'(z) J_z) from the pre-activation z and the Jacobian rows J_z = a[1..3] of the GEMM's a[], and
+// stores it as the next layer's input in H or, after the last layer, y as the trunk features in F (neus.py:128,145),
+// channel 0's y as the sdf (neus.py:127) and its J_y as the normal rows of X (neus.py:133-142).
+__device__ __forceinline__ float4 sdf_epilogue(const Params& P, float* smem, bool last, int ch, int sg, int col, float z,
+                                               const float (&a)[4]) {
+  float y, d1, d2;
+  act_fdd(P.act, z, y, d1, d2);
+  const float4 o = make_float4(y, d1 * a[1], d1 * a[2], d1 * a[3]);
+  if (!last) {
+    *reinterpret_cast<float4*>(smem + kOffH + ch * kT + 4 * sg) = o;
+  } else {
+    smem[kOffF + ch * kT + col] = y;
+    if (ch == 0) {
+      float* X = smem + kOffX;
+      const int x_normal = 3 + 2 * (3 * P.embed_dir);
+      smem[kOffSdf + col] = y;
+      X[(x_normal + 0) * kT + col] = o.y;
+      X[(x_normal + 1) * kT + col] = o.z;
+      X[(x_normal + 2) * kT + col] = o.w;
+    }
+  }
+  return o;
+}
+
+// colour output layer's pre-activation c of sample s on the colour trunk's last features in H (neus.py:148)
+__device__ __forceinline__ float colour_head_pre(const Params& P, const float* H, int s, int c) {
+  const float* wh = P.w + P.head_off;
+  float a = NEUS_LDG(wh + 3 * kW + c);
+  for (int k = 0; k < kW; ++k) a = fmaf(NEUS_LDG(wh + c * kW + k), H[k * kT + s], a);
+  return a;
+}
+
 // One CTA: tiles cx.block, cx.block + cx.nblocks, ...
 template <class Ctx>
 __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* smem) {
-  float* E = smem + kOffE;
   float* X = smem + kOffX;
   float* H = smem + kOffH;
-  float* F = smem + kOffF;
-  float* geo = smem + kOffGeo;
   float* sdfv = smem + kOffSdf;
   const int tid = cx.tid;
   const int cg = tid & 15, sg = tid >> 4;
   const int64_t n_tiles = (P.n + kT - 1) / kT;
-  const int ehalf = 3 * P.embed_pos;  // rows of the sine block of the position embedding
-  const int dhalf = 3 * P.embed_dir;
-  const int x_normal = 3 + 2 * dhalf;  // first normal row of X
+  const int x_normal = 3 + 2 * (3 * P.embed_dir);  // first normal row of X
   float acc[4][4][4];
 
   for (int64_t tile = cx.block; tile < n_tiles; tile += cx.nblocks) {
     const int64_t n0 = tile * kT;
-    // ---- geometry of the tile's samples (one thread per sample); rows 0..2 of X = position (neus.py:145) ----
-    if (tid < kT) {
-      float pos[3] = {0.f, 0.f, 0.f}, dir[3] = {0.f, 0.f, 1.f}, var[3];
-      const int64_t n = n0 + tid;
-      if (n < P.n) {
-        if (P.dists) {
-          const int64_t b = n / P.n_edges;
-          const int j = (int)(n - b * P.n_edges);
-          const float* row = P.dists + b * P.n_edges;
-          float o[3];
-#pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            o[i] = P.ray_orig[3 * b + i];
-            dir[i] = P.ray_dir[3 * b + i];
-          }
-          sample_geometry(P.sampling_type, P.ray_radius, o, dir, row[j], far_edge(row, j, P.n_edges), pos, var);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            pos[i] = P.pos[3 * n + i];
-            dir[i] = P.dir[3 * n + i];
-          }
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        geo[tid * 6 + i] = pos[i];
-        geo[tid * 6 + 3 + i] = dir[i];
-        X[i * kT + tid] = pos[i];
-      }
-    }
-    cx.sync();
-    // ---- direction embedding into X (neus.py:120): four threads per sample ----
-    {
-      const int s = tid >> 2, sub4 = tid & 3;
-      for (int idx = sub4; idx < dhalf; idx += 4) {
-        const int e = idx / 3, d = idx - 3 * e;
-        float sn, cs;
-        sincosf((float)(1u << e) * geo[s * 6 + 3 + d], &sn, &cs);
-        X[(3 + idx) * kT + s] = sn;
-        X[(3 + dhalf + idx) * kT + s] = cs;
-      }
-    }
-    // (no barrier: X is first read by the colour trunk, behind the barriers of the SDF trunk)
+    prologue(cx, P, smem, n0);
 
     // ---- SDF trunk on four sub-tiles of 16 samples (value + three Jacobian columns per sample) ----
     for (int sub = 0; sub < kT / kSub; ++sub) {
-      // position embedding with its Jacobian (neus.py:119): sixteen threads per sample
-      {
-        const int s = tid >> 4, lane16 = tid & 15;
-        const float* p3 = geo + (kSub * sub + s) * 6;
-        for (int idx = lane16; idx < ehalf; idx += 16) {
-          const int e = idx / 3, d = idx - 3 * e;
-          const float f = (float)(1u << e);
-          float sn, cs;
-          sincosf(f * p3[d], &sn, &cs);
-          float4 vs = make_float4(sn, 0.f, 0.f, 0.f), vc = make_float4(cs, 0.f, 0.f, 0.f);
-          const float js = f * cs, jc = -(f * sn);
-          if (d == 0) { vs.y = js; vc.y = jc; }
-          else if (d == 1) { vs.z = js; vc.z = jc; }
-          else { vs.w = js; vc.w = jc; }
-          *reinterpret_cast<float4*>(E + idx * kT + 4 * s) = vs;
-          *reinterpret_cast<float4*>(E + (ehalf + idx) * kT + 4 * s) = vc;
-        }
-      }
-      cx.sync();
+      sdf_embedding(cx, P, smem, sub);
       for (int l = 0; l < P.n_sdf; ++l) {
         const Layer& L = P.lsdf[l];
         layer_gemm(cx, P, L, smem, acc);
         const float* bl = P.w + L.b_off;
         const bool last = (l == P.n_sdf - 1);
-        const int col = kSub * sub + sg;  // the sample's column in the colour trunk
 #pragma unroll
         for (int i = 0; i < 4; ++i)
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             const int ch = 4 * cg + 64 * i + j;
-            float y, d1;
-            act_fd(P.act, acc[i][j][0] + NEUS_LDG(bl + ch), y, d1);
-            const float4 o = make_float4(y, d1 * acc[i][j][1], d1 * acc[i][j][2], d1 * acc[i][j][3]);
-            if (!last) {
-              *reinterpret_cast<float4*>(H + ch * kT + 4 * sg) = o;
-            } else {
-              F[ch * kT + col] = y;  // trunk features of the colour input (neus.py:128,145)
-              if (ch == 0) {         // sdf = channel 0 (neus.py:127), normal = its Jacobian column (neus.py:133-142)
-                sdfv[col] = y;
-                X[(x_normal + 0) * kT + col] = o.y;
-                X[(x_normal + 1) * kT + col] = o.z;
-                X[(x_normal + 2) * kT + col] = o.w;
-              }
-            }
+            sdf_epilogue(P, smem, last, ch, sg, kSub * sub + sg, acc[i][j][0] + NEUS_LDG(bl + ch), acc[i][j]);
           }
         cx.sync();
       }
@@ -270,26 +302,23 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
           const int ch = 4 * cg + 64 * i + j;
           const float b = NEUS_LDG(bl + ch);
           float4 o;
-          float d1;
-          act_fd(P.act, acc[i][j][0] + b, o.x, d1);
-          act_fd(P.act, acc[i][j][1] + b, o.y, d1);
-          act_fd(P.act, acc[i][j][2] + b, o.z, d1);
-          act_fd(P.act, acc[i][j][3] + b, o.w, d1);
+          float d1, d2;
+          act_fdd(P.act, acc[i][j][0] + b, o.x, d1, d2);
+          act_fdd(P.act, acc[i][j][1] + b, o.y, d1, d2);
+          act_fdd(P.act, acc[i][j][2] + b, o.z, d1, d2);
+          act_fdd(P.act, acc[i][j][3] + b, o.w, d1, d2);
           *reinterpret_cast<float4*>(H + ch * kT + 4 * sg) = o;
         }
       cx.sync();
     }
     // ---- colour output layer + activation (neus.py:148-149: the activation follows the last layer too) ----
     if (tid < kT) {
-      const float* wh = P.w + P.head_off;
       const int64_t n = n0 + tid;
       float o[3];
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
-        float a = NEUS_LDG(wh + 3 * kW + c);
-        for (int k = 0; k < kW; ++k) a = fmaf(NEUS_LDG(wh + c * kW + k), H[k * kT + tid], a);
-        float d1;
-        act_fd(P.act, a, o[c], d1);
+        float d1, d2;
+        act_fdd(P.act, colour_head_pre(P, H, tid, c), o[c], d1, d2);
       }
       if (n < P.n) {
         P.color[3 * n + 0] = o[0];
@@ -301,11 +330,31 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
   }
 }
 
-#ifdef __CUDACC__
-// colour output layer [3][256] + 3 biases as stored by torch, and the variance parameter (neus_simt.cu)
-__global__ void neus_pack_head_kernel(const float* __restrict__ wc, const float* __restrict__ bc, const float* __restrict__ variance,
-                                      float* __restrict__ dst_head, float* __restrict__ dst_var);
-#endif
+// torch's tensors in the order of layer_shapes, and the variance parameter
+struct Tensors : simt::Linears<kMaxSdf + kMaxCol + 2> {
+  const float* variance;
+};
+
+// Packs t into the buffer laid out by build_program (work items t0, t0 + stride, ... as simt::pack_linear): every
+// layer's forward pack and bias, the colour output layer [3][256] + 3 biases as stored by torch, the variance.
+// wt_sdf / wt_col: offsets of the training backward's transposed packs (neust::build_program; wt_sdf[0] unused), or
+// nullptr for the forward's buffer.
+__device__ __forceinline__ void pack(int t0, int stride, const Params& P, const int* wt_sdf, const int* wt_col, const Tensors& t,
+                                     float* dst) {
+  const int n_x = 6 + 6 * P.embed_dir;
+  for (int i = 0; i < P.n_sdf + P.n_col; ++i) {
+    const bool sdf = i < P.n_sdf;
+    const int l = sdf ? i : i - P.n_sdf;
+    const Layer& ly = sdf ? P.lsdf[l] : P.lcol[l];
+    const bool tr = wt_sdf && (!sdf || l > 0);  // transposed pack over the h part (colour layer 0: the F part)
+    simt::pack_linear(t0, stride, t.w[i], t.b[i], t.n_in[i], t.n_out[i], ly.k_pad, tr ? kW : 0, (!sdf && l == 0) ? n_x : 0,
+                      dst + ly.w_off, dst + ly.b_off, tr ? dst + (sdf ? wt_sdf[l] : wt_col[l]) : nullptr);
+  }
+  const int h = P.n_sdf + P.n_col;
+  for (int i = t0; i < 3 * kW; i += stride) dst[P.head_off + i] = t.w[h][i];
+  for (int i = t0; i < 3; i += stride) dst[P.head_off + 3 * kW + i] = t.b[h][i];
+  if (t0 == 0) dst[P.var_off] = t.variance[0];
+}
 
 // ---------------------------------------------------------------------------------------------
 // host: layer table from the constructor arguments (neus.py:83-98)

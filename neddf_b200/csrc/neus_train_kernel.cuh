@@ -7,9 +7,7 @@
 // is reverse mode through a forward-mode trunk.  Per SDF layer, z = x W + b, J_z = J_x W, y = f(z), J_y = f'(z) J_z:
 //     g_z = g_y f'(z) + sum_i g_Jy_i J_z_i f''(z),   g_Jz_i = g_Jy_i f'(z),   (g_x, g_Jx_i) = (g_z, g_Jz_i) W^T
 //     gW = x^T g_z + sum_i J_x_i^T g_Jz_i  (a GEMM over the four rows of every sample),   gb = sum g_z
-// f'' is the reference's: its tanhExp (nn_module/tanh_exp.py) saves ex = exp(x), tx = tanh(ex) without a graph inside
-// forward, so double backward differentiates its backward d = tx - x ex (tx^2 - 1) through the explicit x only:
-// f''_ref = ex (1 - tx^2) (0 above the threshold 20), not the true second derivative.  ReLU: f'' = 0.
+// f'' is the reference's, not the true second derivative (neus::act_fdd).
 // Sources at the end of the SDF trunk: colour layer 0 reads [pos | dir PE | normal | F] - its input gradient feeds the
 // Jacobian rows of channel 0 (normal) and the value rows of all channels (F); density = 10 v e / (1 + e)^2,
 // e = exp(-10 v sdf), feeds channel 0's value row and `variance`; upstream gradients of the returned sdf / normal, if
@@ -17,8 +15,9 @@
 // output too (neus.py:148-149).
 //
 // One kernel per backward call, per 64-sample tile:
-//   phase 1  the forward of neus_kernel.cuh (same geometry, embeddings, layer table, 16-sample x 4-column SDF
-//            sub-tiles, GEMM loop), parking every SDF layer's (z, J_z) in the slot of its gradient buffer GS[l] and its
+//   phase 1  the forward of neus_kernel.cuh - its layer table, prologue, position embedding, GEMM, SDF epilogue,
+//            activation and colour head - so the backward differentiates the very values the forward returned;
+//            parking every SDF layer's (z, J_z) in the slot of its gradient buffer GS[l] and its
 //            output (y, J_y) in XS[l]; every colour layer's z in GC[l] and h in XC[l]; the colour input [pos | dir PE |
 //            normal] in XC0, the trunk features in FO; the embedding with its Jacobian rows in E4.
 //   phase 2  head gradient, colour trunk backward over the 64 samples (transposed packs), the F and normal parts of
@@ -40,10 +39,9 @@ using neus::kSub;
 using neus::kT;
 using neus::kThreads;
 using neus::kW;
-using simt::pack_t;
 
 struct Params {
-  neus::Params f;           // network (forward packs, layer table) and sample geometry; f's outputs are unused
+  neus::Params f;             // network (forward packs, layer table) and sample geometry; f's outputs are unused
   int wt_sdf[neus::kMaxSdf];  // SDF layer l >= 1: transposed pack [256 outputs][256 inputs of the h part]
   int wt_col[neus::kMaxCol];  // colour layer l >= 1: [256][256]; colour layer 0: the F part of its input
   int n_e, n_x;             // 6 embed_pos_rank; 6 + 6 embed_dir_rank
@@ -67,26 +65,6 @@ constexpr int kOffGH = kOffUp + kT * 8;    // [kT][4] head pre-activation gradie
 constexpr int kOffGN = kOffGH + kT * 4;    // [kT][4] gradient of the normal (colour layer 0 + upstream)
 constexpr int kSmemFloats = kOffGN + kT * 4;
 constexpr size_t kSmemBytes = (size_t)kSmemFloats * sizeof(float);
-
-// value, slope and the reference's second derivative (header comment) of the NeuS activations
-__device__ __forceinline__ void act_fdd(int act, float x, float& y, float& d1, float& d2) {
-  if (act == NEDDF_ACT_TANHEXP) {
-    const float ex = expf(x);
-    const float tx = tanhf(ex);
-    y = x * tx;
-    d1 = tx - x * ex * (tx * tx - 1.0f);
-    d2 = ex * (1.0f - tx * tx);
-    if (x > 20.0f) {
-      y = x;
-      d1 = 1.0f;
-      d2 = 0.0f;
-    }
-  } else {
-    d1 = (x > 0.0f) ? 1.0f : 0.0f;
-    y = (x > 0.0f) ? x : 0.0f;
-    d2 = 0.0f;
-  }
-}
 
 // d density / d sdf and d density / d variance of neus.py:150-153 (a = 10 v, e = exp(-a s), r = 1 / (1 + e),
 // density = a e r^2): d/ds = -a^2 (e r) r (2 r - 1), d/dv = 10 (e r) r (1 - a s (2 r - 1)); e r = 1 - r where e > 1
@@ -118,111 +96,56 @@ __device__ __forceinline__ neus::Layer transposed(int wt_off) {
 template <class Ctx>
 __device__ __forceinline__ void tile_program(Ctx& cx, const Params& T, float* smem) {
   const neus::Params& P = T.f;
-  float* E = smem + neus::kOffE;
-  float* X = smem + neus::kOffX;
+  const float* E = smem + neus::kOffE;
+  const float* X = smem + neus::kOffX;
   float* H = smem + neus::kOffH;
   float* F = smem + neus::kOffF;
-  float* geo = smem + neus::kOffGeo;
-  float* sdfv = smem + neus::kOffSdf;
+  const float* sdfv = smem + neus::kOffSdf;
   float* up = smem + kOffUp;
   float* gh = smem + kOffGH;
   float* gn = smem + kOffGN;
   const int tid = cx.tid;
   const int cg = tid & 15, sg = tid >> 4;
   const int64_t n_tiles = (P.n + kT - 1) / kT;
-  const int ehalf = 3 * P.embed_pos;
-  const int dhalf = 3 * P.embed_dir;
-  const int x_normal = 3 + 2 * dhalf;
+  const int x_normal = 3 + 2 * (3 * P.embed_dir);
   const int n_e = T.n_e, n_x = T.n_x;
   const int Ls = P.n_sdf, Lc = P.n_col;
   float acc[4][4][4];
 
   for (int64_t tile = cx.block; tile < n_tiles; tile += cx.nblocks) {
     const int64_t n0 = tile * kT;
-    // ---- geometry + upstream gradients (one thread per sample); rows 0..2 of X = position ----
+    neus::prologue(cx, P, smem, n0);
+    // upstream gradients of the tile's samples (one thread per sample): no barrier, as they are first read behind the
+    // barriers of phase 1 (by the thread that wrote them in the colour head, by others in phase 2)
     if (tid < kT) {
-      float pos[3] = {0.f, 0.f, 0.f}, dir[3] = {0.f, 0.f, 1.f}, var[3];
       float u[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
       const int64_t n = n0 + tid;
       if (n < P.n) {
-        if (P.dists) {
-          const int64_t b = n / P.n_edges;
-          const int j = (int)(n - b * P.n_edges);
-          const float* row = P.dists + b * P.n_edges;
-          float o[3];
-#pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            o[i] = P.ray_orig[3 * b + i];
-            dir[i] = P.ray_dir[3 * b + i];
-          }
-          sample_geometry(P.sampling_type, P.ray_radius, o, dir, row[j], far_edge(row, j, P.n_edges), pos, var);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            pos[i] = P.pos[3 * n + i];
-            dir[i] = P.dir[3 * n + i];
-          }
-        }
 #pragma unroll
         for (int i = 0; i < 3; ++i) u[i] = T.g_color[3 * n + i];
         u[3] = T.g_density[n];
         u[4] = T.g_sdf ? T.g_sdf[n] : 0.f;
       }
 #pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        geo[tid * 6 + i] = pos[i];
-        geo[tid * 6 + 3 + i] = dir[i];
-        X[i * kT + tid] = pos[i];
-      }
-#pragma unroll
       for (int i = 0; i < 8; ++i) up[tid * 8 + i] = u[i];
-    }
-    cx.sync();
-    // ---- direction embedding into X: four threads per sample ----
-    {
-      const int s = tid >> 2, sub4 = tid & 3;
-      for (int idx = sub4; idx < dhalf; idx += 4) {
-        const int e = idx / 3, d = idx - 3 * e;
-        float sn, cs;
-        sincosf((float)(1u << e) * geo[s * 6 + 3 + d], &sn, &cs);
-        X[(3 + idx) * kT + s] = sn;
-        X[(3 + dhalf + idx) * kT + s] = cs;
-      }
     }
 
     // ================================ phase 1: forward, parking z / J_z and y / J_y ================================
     for (int sub = 0; sub < kT / kSub; ++sub) {
-      {
-        const int s = tid >> 4, lane16 = tid & 15;
-        const float* p3 = geo + (kSub * sub + s) * 6;
-        for (int idx = lane16; idx < ehalf; idx += 16) {
-          const int e = idx / 3, d = idx - 3 * e;
-          const float f = (float)(1u << e);
-          float sn, cs;
-          sincosf(f * p3[d], &sn, &cs);
-          float4 vs = make_float4(sn, 0.f, 0.f, 0.f), vc = make_float4(cs, 0.f, 0.f, 0.f);
-          const float js = f * cs, jc = -(f * sn);
-          if (d == 0) { vs.y = js; vc.y = jc; }
-          else if (d == 1) { vs.z = js; vc.z = jc; }
-          else { vs.w = js; vc.w = jc; }
-          *reinterpret_cast<float4*>(E + idx * kT + 4 * s) = vs;
-          *reinterpret_cast<float4*>(E + (ehalf + idx) * kT + 4 * s) = vc;
-        }
-      }
-      cx.sync();
+      neus::sdf_embedding(cx, P, smem, sub);
       // the embedding rows as a GEMM operand: E4[n][r][k]
       for (int idx = tid; idx < kSub * 4 * n_e; idx += kThreads) {
         const int s = idx / (4 * n_e), rk = idx - s * 4 * n_e, r = rk / n_e, k = rk - r * n_e;
         const int64_t n = n0 + kSub * sub + s;
         if (n < P.n) T.E4[n * 4 * n_e + rk] = E[k * kT + 4 * s + r];
       }
-      const int64_t n_me = n0 + kSub * sub + sg;  // this thread's sample in the epilogues
+      const int col = kSub * sub + sg;
+      const int64_t n_me = n0 + col;  // this thread's sample in the epilogues
       for (int l = 0; l < Ls; ++l) {
         const neus::Layer& L = P.lsdf[l];
         neus::layer_gemm(cx, P, L, smem, acc);
         const float* bl = P.w + L.b_off;
         const bool last = (l == Ls - 1);
-        const int col = kSub * sub + sg;
         float* Gl = T.GS + (size_t)l * P.n * 4 * kW;
         float* Xl = T.XS + (size_t)l * P.n * 4 * kW;
 #pragma unroll
@@ -231,28 +154,15 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& T, float* sm
           float z[4][4], o[4][4];  // [j][row]
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
-            const int ch = ch0 + j;
-            float y, d1;
-            z[j][0] = acc[i][j][0] + NEUS_LDG(bl + ch);
+            z[j][0] = acc[i][j][0] + NEUS_LDG(bl + ch0 + j);
             z[j][1] = acc[i][j][1];
             z[j][2] = acc[i][j][2];
             z[j][3] = acc[i][j][3];
-            neus::act_fd(P.act, z[j][0], y, d1);
-            o[j][0] = y;
-            o[j][1] = d1 * acc[i][j][1];
-            o[j][2] = d1 * acc[i][j][2];
-            o[j][3] = d1 * acc[i][j][3];
-            if (!last) {
-              *reinterpret_cast<float4*>(H + ch * kT + 4 * sg) = make_float4(o[j][0], o[j][1], o[j][2], o[j][3]);
-            } else {
-              F[ch * kT + col] = y;
-              if (ch == 0) {
-                sdfv[col] = y;
-                X[(x_normal + 0) * kT + col] = o[j][1];
-                X[(x_normal + 1) * kT + col] = o[j][2];
-                X[(x_normal + 2) * kT + col] = o[j][3];
-              }
-            }
+            const float4 y = neus::sdf_epilogue(P, smem, last, ch0 + j, sg, col, z[j][0], acc[i][j]);
+            o[j][0] = y.x;
+            o[j][1] = y.y;
+            o[j][2] = y.z;
+            o[j][3] = y.w;
           }
           if (n_me < P.n) {
 #pragma unroll
@@ -290,9 +200,9 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& T, float* sm
           const float b = NEUS_LDG(bl + ch0 + j);
 #pragma unroll
           for (int s = 0; s < 4; ++s) {
-            float d1;
+            float d1, d2;
             z[j][s] = acc[i][j][s] + b;
-            neus::act_fd(P.act, z[j][s], h[j][s], d1);
+            neus::act_fdd(P.act, z[j][s], h[j][s], d1, d2);
           }
           *reinterpret_cast<float4*>(H + (ch0 + j) * kT + 4 * sg) = make_float4(h[j][0], h[j][1], h[j][2], h[j][3]);
         }
@@ -309,14 +219,11 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& T, float* sm
     }
     // ---- colour output layer: g_zh = g_color act'(z_h) ----
     if (tid < kT) {
-      const float* wh = P.w + P.head_off;
       const int64_t n = n0 + tid;
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
-        float a = NEUS_LDG(wh + 3 * kW + c);
-        for (int k = 0; k < kW; ++k) a = fmaf(NEUS_LDG(wh + c * kW + k), H[k * kT + tid], a);
-        float y, d1;
-        neus::act_fd(P.act, a, y, d1);
+        float y, d1, d2;
+        neus::act_fdd(P.act, neus::colour_head_pre(P, H, tid, c), y, d1, d2);
         const float g = up[tid * 8 + c] * d1;
         gh[tid * 4 + c] = g;
         if (n < P.n) T.GH[n * 3 + c] = g;
@@ -357,8 +264,8 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& T, float* sm
           const float zz[4] = {z4.x, z4.y, z4.z, z4.w};
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
-            float y, d1;
-            neus::act_fd(P.act, zz[j], y, d1);
+            float y, d1, d2;
+            neus::act_fdd(P.act, zz[j], y, d1, d2);
             gz[j][s] = acc[i][j][s] * d1;
           }
           if (n < P.n) *reinterpret_cast<float4*>(Gl + n * kW + ch0) = make_float4(gz[0][s], gz[1][s], gz[2][s], gz[3][s]);
@@ -434,7 +341,7 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& T, float* sm
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             float y, d1, d2;
-            act_fdd(P.act, zr[0][j], y, d1, d2);
+            neus::act_fdd(P.act, zr[0][j], y, d1, d2);
             const float gy = acc[i][j][0], gj1 = acc[i][j][1], gj2 = acc[i][j][2], gj3 = acc[i][j][3];
             g[0][j] = fmaf(gy, d1, d2 * fmaf(gj3, zr[3][j], fmaf(gj2, zr[2][j], gj1 * zr[1][j])));
             g[1][j] = gj1 * d1;
@@ -455,7 +362,12 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& T, float* sm
   }
 }
 
-// fills T.f (the forward program) and the transposed packs; returns the floats of the packed weight buffer
+#ifdef __CUDACC__
+// the network part of the parameters (simt::Handle)
+inline neus::Params& net(Params& T) { return T.f; }
+#endif
+
+// fills the forward program (T.f) and the transposed packs; returns the floats of the packed weight buffer
 inline size_t build_program(const neddf_neus_config_t* c, Params& T) {
   size_t off = neus::build_program(c, T.f);
   off = (off + 3) / 4 * 4;  // 16-byte aligned packs for cp.async

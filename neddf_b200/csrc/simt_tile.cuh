@@ -13,6 +13,11 @@
 
 #include "common.cuh"
 
+#ifdef __CUDACC__
+#include <algorithm>
+#include <cstring>
+#endif
+
 namespace neddf {
 namespace simt {
 
@@ -102,7 +107,7 @@ __device__ __forceinline__ float pack_t(const float* w, int n_in, int n_out, int
 
 // One torch nn.Linear (weight [n_out][n_in], bias [n_out]) -> forward pack [k_pad][256], bias [256] and, if
 // kt_pad > 0, the transposed pack [kt_pad][256] over the input channels c0 .. c0 + 255.  Work items t0, t0 + stride,
-// ...: the pack kernel below runs it on every thread of its grid, the host emulations on one thread.
+// ...: a network's pack kernel runs it on every thread of its grid, the host emulations on one thread.
 __device__ __forceinline__ void pack_linear(int t0, int stride, const float* w, const float* b, int n_in, int n_out, int k_pad,
                                             int kt_pad, int c0, float* dst_w, float* dst_b, float* dst_wt) {
   for (int idx = t0; idx < k_pad * kW; idx += stride) dst_w[idx] = pack_entry(w, n_in, n_out, idx / kW, idx % kW);
@@ -110,11 +115,103 @@ __device__ __forceinline__ void pack_linear(int t0, int stride, const float* w, 
   for (int c = t0; c < kW; c += stride) dst_b[c] = c < n_out ? b[c] : 0.f;
 }
 
+// A network's torch tensors in the order of its layer_shapes (weight [n_out][n_in], bias [n_out]), by value so that
+// a pack kernel can take them as a parameter.
+template <int N>
+struct Linears {
+  const float* w[N];
+  const float* b[N];
+  int n_in[N], n_out[N];
+  void set(int n, const float* const* w_, const float* const* b_) {
+    for (int i = 0; i < n; ++i) {
+      w[i] = w_[i];
+      b[i] = b_[i];
+    }
+  }
+};
+
 #ifdef __CUDACC__
-static __global__ void pack_linear_kernel(const float* __restrict__ w, const float* __restrict__ b, int n_in, int n_out, int k_pad,
-                                          int kt_pad, int c0, float* __restrict__ dst_w, float* __restrict__ dst_b,
-                                          float* __restrict__ dst_wt) {
-  pack_linear(blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x, w, b, n_in, n_out, k_pad, kt_pad, c0, dst_w, dst_b, dst_wt);
+// The network part of a kernel's parameters (.w the packed weights, .n the samples): the parameters themselves, unless
+// an overload in the kernel's namespace says otherwise (neust::net).
+template <class Prm>
+Prm& net(Prm& P) {
+  return P;
+}
+
+// ---------------------------------------------------------------------------------------------
+// The C-ABI handle of a CUDA-core kernel: its configuration, torch's layer shapes, the kernel's
+// parameters with the network part filled at creation (net(proto).w = the packed weights d_w) and the packed weights.
+// The entry points keep their own argument checks and error strings; these are the steps they share.
+// ---------------------------------------------------------------------------------------------
+template <class Cfg, class Prog, class Tensors>
+struct Handle {
+  Cfg cfg;
+  int n_layers = 0;
+  Tensors shapes;  // n_in / n_out of torch's tensors
+  Prog proto;
+  float* d_w = nullptr;
+  size_t w_floats = 0;
+  bool packed = false;
+
+  // After the entry point's checks of cfg and out: layer shapes, program (build(cfg, proto) -> floats of the packed
+  // weights), weight buffer.
+  template <class H, class Build>
+  static int32_t create(const char* who, const Cfg* cfg, H** out, int (*layer_shapes)(const Cfg*, int*, int*), Build build) {
+    H* h = new H();
+    h->cfg = *cfg;
+    h->n_layers = layer_shapes(cfg, h->shapes.n_in, h->shapes.n_out);
+    std::memset(&h->proto, 0, sizeof(h->proto));
+    h->w_floats = build(cfg, h->proto);
+    if (cudaMalloc(&h->d_w, h->w_floats * sizeof(float)) != cudaSuccess) {
+      delete h;
+      return fail(NEDDF_E_CUDA, std::string(who) + ": cudaMalloc failed");
+    }
+    net(h->proto).w = h->d_w;
+    *out = h;
+    return NEDDF_OK;
+  }
+
+  template <class H>
+  static void destroy(H* h) {
+    if (!h) return;
+    cudaFree(h->d_w);
+    delete h;
+  }
+
+  // After the entry point's checks of its arguments: packs torch's n_layers tensors w, b (with the shapes and any other
+  // fields of t) into d_w on 64 x 256 threads.
+  template <class Kernel>
+  int32_t pack(Kernel kernel, Tensors t, const float* const* w, const float* const* b, void* stream) {
+    t.set(n_layers, w, b);
+    kernel<<<64, 256, 0, (cudaStream_t)stream>>>(proto, t, d_w);
+    NEDDF_LAUNCH_CHECK();
+    packed = true;
+    return NEDDF_OK;
+  }
+
+  // Guarded persistent launch of `kernel` over net(P).n samples, grid = min(tiles, SMs): refuses weights never set, then
+  // whatever `check` returns (the entry point's remaining argument checks, which may complete P), does nothing for no
+  // samples.
+  template <class Prm, class Check>
+  int32_t launch(const char* who, void (*kernel)(Prm), size_t smem_bytes, Prm& P, void* stream, Check check) const {
+    if (!packed) return fail(NEDDF_E_INVALID, std::string(who) + ": weights were never set");
+    if (int32_t rc = check()) return rc;
+    const int64_t n = net(P).n;
+    if (n <= 0) return NEDDF_OK;
+    const int64_t n_tiles = (n + kT - 1) / kT;
+    const int grid = (int)std::min<int64_t>(n_tiles, sm_count());
+    NEDDF_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    kernel<<<grid, kThreads, smem_bytes, (cudaStream_t)stream>>>(P);
+    NEDDF_LAUNCH_CHECK();
+    return NEDDF_OK;
+  }
+};
+
+// n_edges / sampling_type of the _rays entry points
+inline int32_t check_rays(const char* who, int32_t n_edges, int32_t sampling_type) {
+  if (n_edges < 1 || (sampling_type != NEDDF_SAMPLING_POINT && sampling_type != NEDDF_SAMPLING_CONE))
+    return fail(NEDDF_E_INVALID, std::string(who) + ": bad n_edges / sampling_type");
+  return NEDDF_OK;
 }
 #endif
 

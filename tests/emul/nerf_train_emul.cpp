@@ -7,24 +7,6 @@
 
 using namespace neddf;
 
-// neddf_nerf_set_weights / neddf_nerf_train_set_weights (nerf::pack_weights): simt::pack_linear_kernel per layer,
-// nerf_pack_heads_kernel
-static std::vector<float> pack(const nerf::Params& P, size_t w_floats, const int* sin, const int* sout, const float* const* w,
-                               const float* const* b) {
-  std::vector<float> packed(w_floats, 0.f);
-  const int L = P.n_layers;
-  for (int l = 0; l <= L; ++l) {
-    const int t = (l < L) ? l : L + 1;
-    const nerf::Layer& ly = P.layer[l];
-    simt::pack_linear(0, 1, w[t], b[t], sin[t], sout[t], ly.k_pad, ly.kt_pad, 0, &packed[ly.w_off], &packed[ly.b_off], &packed[ly.wt_off]);
-  }
-  for (int i = 0; i < nerf::kW; ++i) packed[P.w_density_off + i] = w[L][i];
-  packed[P.w_density_off + nerf::kW] = b[L][0];
-  for (int i = 0; i < 3 * (nerf::kW / 2); ++i) packed[P.w_col2_off + i] = w[L + 2][i];
-  for (int i = 0; i < 3; ++i) packed[P.w_col2_off + 3 * (nerf::kW / 2) + i] = b[L + 2][i];
-  return packed;
-}
-
 // The network part of P and its packed weights; then the samples: explicit (pos / dir / var, n = samples) or rays
 // (n = rays).  Returns 0, -1 for a configuration the handle refuses, -2 for a wrong number of tensors.
 static int setup(const neddf_nerf_config_t* cfg, bool training, const float* const* w, const float* const* b,
@@ -35,9 +17,11 @@ static int setup(const neddf_nerf_config_t* cfg, bool training, const float* con
   if (training ? nerft::unsupported(cfg) != nullptr : nerf::unsupported(cfg, code) != nullptr) return -1;
   memset(&P, 0, sizeof(P));
   const size_t w_floats = nerf::build_program(cfg, P, training);
-  int sin[nerf::kMaxLayers + 3], sout[nerf::kMaxLayers + 3];
-  if (nerf::layer_shapes(cfg, sin, sout) != n_layers) return -2;
-  packed = pack(P, w_floats, sin, sout, w, b);
+  nerf::Tensors t{};
+  if (nerf::layer_shapes(cfg, t.n_in, t.n_out) != n_layers) return -2;
+  t.set(n_layers, w, b);
+  packed.assign(w_floats, 0.f);
+  nerf::pack(0, 1, P, t, packed.data());  // neddf_nerf_set_weights / neddf_nerf_train_set_weights
   P.w = packed.data();
   for (int e = 0; e < cfg->embed_pos_rank; ++e) P.lowpass[e] = lowpass[e];
   if (dists) {

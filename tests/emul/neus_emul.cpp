@@ -22,17 +22,12 @@ extern "C" int neus_emul_forward(const neddf_neus_config_t* cfg, const float* co
   neus::Params P;
   memset(&P, 0, sizeof(P));
   const size_t w_floats = neus::build_program(cfg, P);
-  int sin[neus::kMaxSdf + neus::kMaxCol + 2], sout[neus::kMaxSdf + neus::kMaxCol + 2];
-  if (neus::layer_shapes(cfg, sin, sout) != n_layers) return -2;
+  neus::Tensors t{};
+  if (neus::layer_shapes(cfg, t.n_in, t.n_out) != n_layers) return -2;
+  t.set(n_layers, w, b);
+  t.variance = variance;
   std::vector<float> packed(w_floats, 0.f);
-  // neddf_neus_set_weights: simt::pack_linear_kernel per layer, neus_pack_head_kernel
-  for (int t = 0; t < n_layers - 1; ++t) {
-    const neus::Layer& ly = (t < P.n_sdf) ? P.lsdf[t] : P.lcol[t - P.n_sdf];
-    simt::pack_linear(0, 1, w[t], b[t], sin[t], sout[t], ly.k_pad, 0, 0, &packed[ly.w_off], &packed[ly.b_off], nullptr);
-  }
-  for (int i = 0; i < 3 * neus::kW; ++i) packed[P.head_off + i] = w[n_layers - 1][i];
-  for (int i = 0; i < 3; ++i) packed[P.head_off + 3 * neus::kW + i] = b[n_layers - 1][i];
-  packed[P.var_off] = variance[0];
+  neus::pack(0, 1, P, nullptr, nullptr, t, packed.data());  // neddf_neus_set_weights
   P.w = packed.data();
   if (dists) {
     P.n = n * n_edges;

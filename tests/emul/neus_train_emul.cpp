@@ -18,22 +18,13 @@ extern "C" int neus_train_emul(const neddf_neus_config_t* cfg, const float* cons
   neust::Params T;
   memset(&T, 0, sizeof(T));
   const size_t w_floats = neust::build_program(cfg, T);
-  neus::Params& P = T.f;
-  int sin[neus::kMaxSdf + neus::kMaxCol + 2], sout[neus::kMaxSdf + neus::kMaxCol + 2];
-  if (neus::layer_shapes(cfg, sin, sout) != n_layers) return -2;
+  neus::Tensors t{};
+  if (neus::layer_shapes(cfg, t.n_in, t.n_out) != n_layers) return -2;
+  t.set(n_layers, w, b);
+  t.variance = variance;
   std::vector<float> packed(w_floats, 0.f);
-  // neddf_neus_train_set_weights: simt::pack_linear_kernel per layer, neus_pack_head_kernel
-  for (int t = 0; t < n_layers - 1; ++t) {
-    const bool sdf = t < P.n_sdf;
-    const int l = sdf ? t : t - P.n_sdf;
-    const neus::Layer& ly = sdf ? P.lsdf[l] : P.lcol[l];
-    float* wt = sdf ? (l > 0 ? &packed[T.wt_sdf[l]] : nullptr) : &packed[T.wt_col[l]];
-    const int c0 = (!sdf && l == 0) ? T.n_x : 0;
-    simt::pack_linear(0, 1, w[t], b[t], sin[t], sout[t], ly.k_pad, wt ? neus::kW : 0, c0, &packed[ly.w_off], &packed[ly.b_off], wt);
-  }
-  for (int i = 0; i < 3 * neus::kW; ++i) packed[P.head_off + i] = w[n_layers - 1][i];
-  for (int i = 0; i < 3; ++i) packed[P.head_off + 3 * neus::kW + i] = b[n_layers - 1][i];
-  packed[P.var_off] = variance[0];
+  neus::pack(0, 1, T.f, T.wt_sdf, T.wt_col, t, packed.data());  // neddf_neus_train_set_weights
+  neus::Params& P = T.f;
   P.w = packed.data();
   if (dists) {
     P.n = n * n_edges;
