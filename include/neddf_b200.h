@@ -357,6 +357,18 @@ int32_t neddf_nerf_forward_rays(const neddf_nerf_t* h, const float* lowpass, con
                                 const float* d_dists, int64_t n_rays, int32_t n_edges, int32_t sampling_type,
                                 float ray_radius, float* d_density, float* d_color, void* stream);
 
+/* Early ray termination (as neddf_field_forward_rays_segment): the network on ONE depth segment, samples
+ * [edge0, edge0+seg_len) of the rays listed in d_ray_index[0 .. *d_n_active) (both NULL = all n_rays rays); density /
+ * colour are scattered to [ray, edge] of the full [n_rays, n_edges] arrays, which the caller zero-fills: a sample that
+ * is never evaluated has density 0 and contributes nothing to neddf_composite.  *d_n_active is read on the device.
+ * Each evaluated entry equals neddf_nerf_forward_rays' bit for bit.  NEDDF_E_INVALID unless 0 <= edge0, 1 <= seg_len,
+ * edge0 + seg_len <= n_edges and d_ray_index / d_n_active are both given or both NULL. */
+int32_t neddf_nerf_forward_rays_segment(const neddf_nerf_t* h, const float* lowpass, const float* d_ray_dir,
+                                        const float* d_ray_orig, const float* d_dists, int64_t n_rays, int32_t n_edges,
+                                        int32_t sampling_type, float ray_radius, int32_t edge0, int32_t seg_len,
+                                        const int32_t* d_ray_index, const int32_t* d_n_active, float* d_density,
+                                        float* d_color, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * NeuS field variant (SURVEY 8(f) item 3; neddf/network/neus.py).  Forward only, fp32 CUDA-core kernel
  * (csrc/neus_simt.cu + csrc/neus_kernel.cuh); the normal d sdf / d position, which the reference takes with
@@ -402,6 +414,15 @@ int32_t neddf_neus_forward(const neddf_neus_t* h, const float* d_pos, const floa
 int32_t neddf_neus_forward_rays(const neddf_neus_t* h, const float* d_ray_dir, const float* d_ray_orig, const float* d_dists,
                                 int64_t n_rays, int32_t n_edges, int32_t sampling_type, float ray_radius, float* d_sdf,
                                 float* d_density, float* d_color, float* d_normal, void* stream);
+
+/* Early ray termination: the contract of neddf_nerf_forward_rays_segment (one depth segment of the listed rays,
+ * density / colour scattered to [ray, edge] of zero-filled [n_rays, n_edges] arrays, *d_n_active read on the device,
+ * the same argument checks).  The SDF trunk and its normal are evaluated as in neddf_neus_forward_rays - the colour
+ * trunk takes the normal - but only density and colour are written. */
+int32_t neddf_neus_forward_rays_segment(const neddf_neus_t* h, const float* d_ray_dir, const float* d_ray_orig,
+                                        const float* d_dists, int64_t n_rays, int32_t n_edges, int32_t sampling_type,
+                                        float ray_radius, int32_t edge0, int32_t seg_len, const int32_t* d_ray_index,
+                                        const int32_t* d_n_active, float* d_density, float* d_color, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * NeRF field variant, training backward (the autograd graph of nerf.py:107-165 with respect to the parameters that

@@ -105,6 +105,7 @@ _SIGNATURES = {
     "neddf_nerf_set_weights": (_I32, [_P, C.POINTER(_P), C.POINTER(_P), _I32, _P]),
     "neddf_nerf_forward": (_I32, [_P, _FP, _P, _P, _P, _I64, _P, _P, _P]),
     "neddf_nerf_forward_rays": (_I32, [_P, _FP, _P, _P, _P, _I64, _I32, _I32, _F, _P, _P, _P]),
+    "neddf_nerf_forward_rays_segment": (_I32, [_P, _FP, _P, _P, _P, _I64, _I32, _I32, _F, _I32, _I32, _P, _P, _P, _P, _P]),
     "neddf_nerf_train_create": (_I32, [C.POINTER(NerfConfig), C.POINTER(_P)]),
     "neddf_nerf_train_destroy": (None, [_P]),
     "neddf_nerf_train_set_weights": (_I32, [_P, C.POINTER(_P), C.POINTER(_P), _I32, _P]),
@@ -116,6 +117,7 @@ _SIGNATURES = {
     "neddf_neus_set_weights": (_I32, [_P, C.POINTER(_P), C.POINTER(_P), _I32, _P, _P]),
     "neddf_neus_forward": (_I32, [_P, _P, _P, _I64, _P, _P, _P, _P, _P]),
     "neddf_neus_forward_rays": (_I32, [_P, _P, _P, _P, _I64, _I32, _I32, _F, _P, _P, _P, _P, _P]),
+    "neddf_neus_forward_rays_segment": (_I32, [_P, _P, _P, _P, _I64, _I32, _I32, _F, _I32, _I32, _P, _P, _P, _P, _P]),
     "neddf_neus_train_create": (_I32, [C.POINTER(NeusConfig), C.POINTER(_P)]),
     "neddf_neus_train_destroy": (None, [_P]),
     "neddf_neus_train_set_weights": (_I32, [_P, C.POINTER(_P), C.POINTER(_P), _I32, _P, _P]),

@@ -66,6 +66,7 @@ struct Params {
   const float *ray_dir, *ray_orig, *dists;
   int n_edges, sampling_type;
   float ray_radius;
+  simt::Segment seg;  // early ray termination (zero: whole rows); n is then the grid's bound rays x seg.len
   // outputs ([n], [n, 3])
   float* density;
   float* color;
@@ -103,8 +104,8 @@ __device__ __forceinline__ void layer_gemm(Ctx& cx, const Params& P, const Layer
   simt::gemm(cx, P.w + L.w_off, L.k_pad, seg_ptr(smem, L.seg_a), L.n_a, seg_ptr(smem, L.seg_b), L.n_b, smem + kOffW, acc);
 }
 
-// Geometry of tile n0's samples (one thread per sample), then the embeddings E and D (nerf.py:133-142, four threads
-// per sample).  Exit: behind a barrier.
+// Geometry of tile n0's samples (one thread per sample; sample n of P.seg's view), then the embeddings E and D
+// (nerf.py:133-142, four threads per sample).  Exit: behind a barrier.
 template <class Ctx>
 __device__ __forceinline__ void prologue(Ctx& cx, const Params& P, float* smem, int64_t n0) {
   float* E = smem + kOffE;
@@ -114,10 +115,11 @@ __device__ __forceinline__ void prologue(Ctx& cx, const Params& P, float* smem, 
   if (tid < kT) {
     float pos[3] = {0.f, 0.f, 0.f}, dir[3] = {0.f, 0.f, 1.f}, var[3] = {0.f, 0.f, 0.f};
     const int64_t n = n0 + tid;
-    if (n < P.n) {
+    if (n < simt::seg_total(P.seg, P.n)) {
       if (P.dists) {
-        const int64_t b = n / P.n_edges;
-        const int j = (int)(n - b * P.n_edges);
+        int64_t b;
+        int j;
+        simt::seg_ray_edge(P.seg, P.n_edges, n, b, j);
         const float* row = P.dists + b * P.n_edges;
         float o[3];
 #pragma unroll
@@ -176,7 +178,8 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
   float* H = smem + kOffH;
   const int tid = cx.tid;
   const int cg = tid & 15, sg = tid >> 4;
-  const int64_t n_tiles = (P.n + kT - 1) / kT;
+  const int64_t n_total = simt::seg_total(P.seg, P.n);
+  const int64_t n_tiles = (n_total + kT - 1) / kT;
   float acc[4][4][4];
 
   for (int64_t tile = cx.block; tile < n_tiles; tile += cx.nblocks) {
@@ -187,7 +190,7 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
         // density head on the trunk's features, before the colour branch overwrites H
         const int64_t n = n0 + tid;
         const float zd = density_pre(P, H, tid);
-        if (n < P.n) P.density[n] = density_act(P.density_act, zd);
+        if (n < n_total) P.density[simt::seg_out(P.seg, P.n_edges, n)] = density_act(P.density_act, zd);
       }
       // (no barrier needed: the layer below starts by reading H and only writes it after its own barriers)
       const Layer& L = P.layer[l];
@@ -221,10 +224,11 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
         for (int k = 0; k < kW / 2; ++k) a = fmaf(NERF_LDG(wc2 + c * (kW / 2) + k), H[k * kT + tid], a);
         o[c] = a;
       }
-      if (n < P.n) {
-        P.color[3 * n + 0] = o[0];
-        P.color[3 * n + 1] = o[1];
-        P.color[3 * n + 2] = o[2];
+      if (n < n_total) {
+        const int64_t on = simt::seg_out(P.seg, P.n_edges, n);
+        P.color[3 * on + 0] = o[0];
+        P.color[3 * on + 1] = o[1];
+        P.color[3 * on + 2] = o[2];
       }
     }
     cx.sync();  // H, E, D, geo are rewritten by the next tile

@@ -72,7 +72,8 @@ struct Params {
   const float *ray_dir, *ray_orig, *dists;
   int n_edges, sampling_type;
   float ray_radius;
-  // outputs ([n], [n], [n,3], optional [n,3])
+  simt::Segment seg;  // early ray termination (zero: whole rows); n is then the grid's bound rays x seg.len
+  // outputs ([n], [n], [n,3], optional [n,3]; sdf optional too, NULL in segment launches)
   float* sdf;
   float* density;
   float* color;
@@ -134,9 +135,9 @@ __device__ __forceinline__ void layer_gemm(Ctx& cx, const Params& P, const Layer
   simt::gemm(cx, P.w + L.w_off, L.k_pad, A, L.n_a, B, L.n_b, smem + kOffW, acc);
 }
 
-// Geometry of tile n0's samples (one thread per sample) into geo and rows 0..2 of X (position, neus.py:145), then the
-// direction embedding into X (neus.py:120, four threads per sample).  Exit: NOT behind a barrier - X is first read by
-// the colour trunk, behind the barriers of the SDF trunk.
+// Geometry of tile n0's samples (one thread per sample; sample n of P.seg's view) into geo and rows 0..2 of X
+// (position, neus.py:145), then the direction embedding into X (neus.py:120, four threads per sample).  Exit: NOT
+// behind a barrier - X is first read by the colour trunk, behind the barriers of the SDF trunk.
 template <class Ctx>
 __device__ __forceinline__ void prologue(Ctx& cx, const Params& P, float* smem, int64_t n0) {
   float* X = smem + kOffX;
@@ -145,10 +146,11 @@ __device__ __forceinline__ void prologue(Ctx& cx, const Params& P, float* smem, 
   if (tid < kT) {
     float pos[3] = {0.f, 0.f, 0.f}, dir[3] = {0.f, 0.f, 1.f}, var[3];
     const int64_t n = n0 + tid;
-    if (n < P.n) {
+    if (n < simt::seg_total(P.seg, P.n)) {
       if (P.dists) {
-        const int64_t b = n / P.n_edges;
-        const int j = (int)(n - b * P.n_edges);
+        int64_t b;
+        int j;
+        simt::seg_ray_edge(P.seg, P.n_edges, n, b, j);
         const float* row = P.dists + b * P.n_edges;
         float o[3];
 #pragma unroll
@@ -249,7 +251,8 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
   float* sdfv = smem + kOffSdf;
   const int tid = cx.tid;
   const int cg = tid & 15, sg = tid >> 4;
-  const int64_t n_tiles = (P.n + kT - 1) / kT;
+  const int64_t n_total = simt::seg_total(P.seg, P.n);
+  const int64_t n_tiles = (n_total + kT - 1) / kT;
   const int x_normal = 3 + 2 * (3 * P.embed_dir);  // first normal row of X
   float acc[4][4][4];
 
@@ -279,13 +282,14 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
     // ---- sdf, density, normal of the tile (neus.py:150-159) ----
     if (tid < kT) {
       const int64_t n = n0 + tid;
-      if (n < P.n) {
+      if (n < n_total) {
+        const int64_t on = simt::seg_out(P.seg, P.n_edges, n);
         const float s = sdfv[tid];
-        P.sdf[n] = s;
-        P.density[n] = sdf_density(s, NEUS_LDG(P.w + P.var_off));
+        if (P.sdf) P.sdf[on] = s;
+        P.density[on] = sdf_density(s, NEUS_LDG(P.w + P.var_off));
         if (P.normal) {
 #pragma unroll
-          for (int i = 0; i < 3; ++i) P.normal[3 * n + i] = X[(x_normal + i) * kT + tid];
+          for (int i = 0; i < 3; ++i) P.normal[3 * on + i] = X[(x_normal + i) * kT + tid];
         }
       }
     }
@@ -320,10 +324,11 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
         float d1, d2;
         act_fdd(P.act, colour_head_pre(P, H, tid, c), o[c], d1, d2);
       }
-      if (n < P.n) {
-        P.color[3 * n + 0] = o[0];
-        P.color[3 * n + 1] = o[1];
-        P.color[3 * n + 2] = o[2];
+      if (n < n_total) {
+        const int64_t on = simt::seg_out(P.seg, P.n_edges, n);
+        P.color[3 * on + 0] = o[0];
+        P.color[3 * on + 1] = o[1];
+        P.color[3 * on + 2] = o[2];
       }
     }
     cx.sync();  // X, H, F, geo, sdfv are rewritten by the next tile

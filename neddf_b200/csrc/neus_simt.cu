@@ -91,3 +91,21 @@ extern "C" int32_t neddf_neus_forward_rays(const neddf_neus_t* h, const float* d
   P.sdf = d_sdf; P.density = d_density; P.color = d_color; P.normal = d_normal;
   return neus_launch(h, P, stream);
 }
+
+extern "C" int32_t neddf_neus_forward_rays_segment(const neddf_neus_t* h, const float* d_ray_dir, const float* d_ray_orig,
+                                                   const float* d_dists, int64_t n_rays, int32_t n_edges, int32_t sampling_type,
+                                                   float ray_radius, int32_t edge0, int32_t seg_len, const int32_t* d_ray_index,
+                                                   const int32_t* d_n_active, float* d_density, float* d_color, void* stream) {
+  const char* who = "neddf_neus_forward_rays_segment";
+  if (!h || !d_ray_dir || !d_ray_orig || !d_dists || !d_density || !d_color) return fail(NEDDF_E_INVALID, std::string(who) + ": null argument");
+  if (int32_t rc = simt::check_rays(who, n_edges, sampling_type)) return rc;
+  simt::Segment seg;
+  if (int32_t rc = simt::check_segment(who, n_edges, edge0, seg_len, d_ray_index, d_n_active, seg)) return rc;
+  neus::Params P = h->proto;
+  P.seg = seg;
+  P.n = n_rays * seg_len;  // bound of the grid; the kernel reads *d_n_active
+  P.ray_dir = d_ray_dir; P.ray_orig = d_ray_orig; P.dists = d_dists;
+  P.n_edges = n_edges; P.sampling_type = sampling_type; P.ray_radius = ray_radius;
+  P.density = d_density; P.color = d_color;  // no sdf / normal outputs (the colour trunk still takes the normal)
+  return neus_launch(h, P, stream);
+}

@@ -223,6 +223,24 @@ class NeRF(BaseNeuralField):
                                                     L.ptr(out["color"]), L.stream_ptr(device)), "nerf_forward_rays")
         return out
 
+    def forward_rays_segment(self, ray_dir: Tensor, ray_orig: Tensor, dists: Tensor, sampling_type: str, ray_radius: float,
+                             edge0: int, seg_len: int, ray_index: Optional[Tensor], n_active: Optional[Tensor],
+                             density: Tensor, color: Tensor) -> None:
+        """One depth segment of the fine pass for early ray termination (neddf_nerf_forward_rays_segment): samples
+        [edge0, edge0 + seg_len) of the rays listed in ``ray_index[:n_active]`` (device tensors, None = all rays);
+        results are scattered into ``density`` [B,E] / ``color`` [B,E,3] in place, equal bit for bit to what
+        ``forward_rays`` gives there.  No-grad only."""
+        self._refuse_autograd("forward_rays_segment")
+        B, E = dists.shape
+        device = dists.device
+        h = self._field(device)
+        # the executed count lives on the device (NeRFRender.termination_stats): no n_evaluations
+        with self._profiled(device, None), torch.cuda.device(device):
+            L.check(L.lib().neddf_nerf_forward_rays_segment(
+                h, self._lowpass(), L.ptr(ray_dir), L.ptr(ray_orig), L.ptr(dists), B, E, L.SAMPLING_IDS[sampling_type],
+                float(ray_radius), int(edge0), int(seg_len), L.ptr(ray_index), L.ptr(n_active), L.ptr(density), L.ptr(color),
+                L.stream_ptr(device)), "nerf_forward_rays_segment")
+
     def set_iter(self, iter: int) -> None:
         """nerf.py:167-178."""
         if iter == -1:

@@ -253,6 +253,12 @@ class BaseNeuralField(nn.Module):
             raise NotImplementedError(self._GRAD_REFUSAL)
         return True
 
+    def _refuse_autograd(self, what: str) -> None:
+        """Raise when autograd is recording for a trainable parameter: ``what`` skips samples and has no gradient."""
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            raise RuntimeError(f"neddf_b200.{type(self).__name__}.{what} evaluates the samples of early ray termination "
+                               "and has no gradient: call it under torch.no_grad() (render_image does)")
+
     @contextlib.contextmanager
     def _profiled(self, device: torch.device, n_evaluations: Optional[int]):
         """Brackets a launch with CUDA events appended to ``_profile_events`` when it is a list."""

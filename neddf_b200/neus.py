@@ -249,3 +249,21 @@ class NeuS(BaseNeuralField):
                                                     L.ptr(out["density"]), L.ptr(out["color"]), L.ptr(out.get("normal")),
                                                     L.stream_ptr(device)), "neus_forward_rays")
         return out
+
+    def forward_rays_segment(self, ray_dir: Tensor, ray_orig: Tensor, dists: Tensor, sampling_type: str, ray_radius: float,
+                             edge0: int, seg_len: int, ray_index: Optional[Tensor], n_active: Optional[Tensor],
+                             density: Tensor, color: Tensor) -> None:
+        """One depth segment of the fine pass for early ray termination (neddf_neus_forward_rays_segment): samples
+        [edge0, edge0 + seg_len) of the rays listed in ``ray_index[:n_active]`` (device tensors, None = all rays);
+        density [B,E] and color [B,E,3] are scattered in place, equal bit for bit to what ``forward_rays`` gives there
+        (the sdf and the normal are evaluated but not returned).  No-grad only."""
+        self._refuse_autograd("forward_rays_segment")
+        B, E = dists.shape
+        device = dists.device
+        h = self._field(device)
+        # the executed count lives on the device (NeRFRender.termination_stats): no n_evaluations
+        with self._profiled(device, None), torch.cuda.device(device):
+            L.check(L.lib().neddf_neus_forward_rays_segment(
+                h, L.ptr(ray_dir), L.ptr(ray_orig), L.ptr(dists), B, E, L.SAMPLING_IDS[sampling_type], float(ray_radius),
+                int(edge0), int(seg_len), L.ptr(ray_index), L.ptr(n_active), L.ptr(density), L.ptr(color),
+                L.stream_ptr(device)), "neus_forward_rays_segment")

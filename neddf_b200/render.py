@@ -298,7 +298,8 @@ class NeRFRender(BaseNeuralRender):
         self.image_chunk = 163840  # 0.76 GB of work buffers; a rank's 80,000- or 160,000-ray shard is one launch sequence
         # Early ray termination (BASELINE.json configs[4]; NOT in the reference, so opt-in): in no-grad image
         # renders the fine pass runs in `termination_segments` depth segments and a ray stops being evaluated
-        # once its transmittance falls to `transmittance_eps`.  0.0 = off = the reference's behaviour, bit for
+        # once its transmittance falls to `transmittance_eps`.  Every fine network of this package has the segment
+        # kernels it needs (NeDDF on all engines, NeRF, NeuS).  0.0 = off = the reference's behaviour, bit for
         # bit.  Error bound: |d color| <= eps * max|c|, |d depth| <= eps * max_dist, |d transmittance| <= eps.
         self.transmittance_eps = 0.0
         self.termination_segments = 4
