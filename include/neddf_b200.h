@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define NEDDF_ABI_VERSION 2
+#define NEDDF_ABI_VERSION 3
 
 #define NEDDF_OK 0
 #define NEDDF_E_INVALID (-1)     /* bad argument / unsupported configuration */
@@ -129,12 +129,15 @@ int32_t neddf_render_loss(const float* d_color, const float* d_color_coarse, con
                           float* g_trans, float* g_trans_coarse, float* g_penalty, float* g_penalty_coarse,
                           void* stream);
 
-/* torch.optim.Adam step of n_tensors parameter tensors in one launch (nerf_trainer.py:38-42, 129); with a
- * field handle the tensors must be (weight, bias) of every layer in reference order and the kernel-layout
- * weights are re-packed on the same stream (what neddf_field_set_weights does after every optimiser step). */
+/* torch.optim.Adam step of n_tensors (1..64) parameter tensors, one launch per 32 tensors (nerf_trainer.py:38-42,
+ * 129), all at the same step count (>= 1); with a field handle the tensors must be (weight, bias) of every layer in
+ * reference order and the kernel-layout weights are re-packed on the same stream (what neddf_field_set_weights does
+ * after every optimiser step).  The betas are doubles because torch rounds `1 - beta` from them, and
+ * 1 - (float)0.999 is 1.3e-5 off.  Without a handle, the pointers of an empty tensor may be NULL.  Every argument is checked before the first launch: a call that returns
+ * NEDDF_E_INVALID has changed no tensor. */
 int32_t neddf_field_adam_step(neddf_field_t* f, float* const* d_params, const float* const* d_grads,
                               float* const* d_exp_avg, float* const* d_exp_avg_sq, const int64_t* h_numel,
-                              int32_t n_tensors, float lr, float beta1, float beta2, float eps, float weight_decay,
+                              int32_t n_tensors, float lr, double beta1, double beta2, float eps, float weight_decay,
                               int64_t step, void* stream);
 
 /* Weight gradients of LinearGradFunction.backward (nn_module/with_grad/linear.py:72-80) as a tensor-core

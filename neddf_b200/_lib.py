@@ -57,7 +57,7 @@ class FieldState(C.Structure):
 
 
 _P = C.c_void_p
-_I32, _I64, _F = C.c_int32, C.c_int64, C.c_float
+_I32, _I64, _F, _D = C.c_int32, C.c_int64, C.c_float, C.c_double
 _FP = C.POINTER(C.c_float)
 
 _SIGNATURES = {
@@ -79,7 +79,7 @@ _SIGNATURES = {
                                         _P, _P, _P, _P, _P, _I32, _I32, _P]),
     "neddf_render_loss": (_I32, [_P] * 8 + [_I64] + [_P] * 8 + [_P]),
     "neddf_field_adam_step": (_I32, [_P, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.POINTER(_P), C.POINTER(_I64), _I32,
-                                     _F, _F, _F, _F, _F, _I64, _P]),
+                                     _F, _D, _D, _F, _F, _I64, _P]),
     "neddf_wgrad_workspace_bytes": (_I64, []),
     "neddf_wgrad": (_I32, [_P, _I64, _I32, _I32, _P, _I64, _I64, _P, _I64, _I32, _P, _P]),
     "neddf_colsum_value_rows": (_I32, [_P, _I64, _I64, _P, _P, _P]),
@@ -166,7 +166,7 @@ def lib():
             fn = getattr(handle, name)  # AttributeError if the ABI lost a symbol
             fn.restype = res
             fn.argtypes = args
-        if handle.neddf_abi_version() != 2:
+        if handle.neddf_abi_version() != 3:
             raise RuntimeError("neddf_b200: ABI version mismatch between Python host and libneddf_b200.so")
         _lib = handle
     return _lib

@@ -92,9 +92,12 @@ struct AdamTensors {
   int count;
 };
 
-// torch.optim.Adam (no amsgrad): m = b1 m + (1 - b1) g; v = b2 v + (1 - b2) g^2;
-// p -= lr / (1 - b1^t) * m / (sqrt(v) / sqrt(1 - b2^t) + eps), with g += weight_decay * p first
-__global__ void adam_kernel(AdamTensors T, float lr, float b1, float b2, float eps, float weight_decay, float bc1, float bc2_sqrt) {
+// torch.optim.Adam (no amsgrad): m = b1 m + (1 - b1) g (as lerp(m, g, 1 - b1)); v = b2 v + (1 - b2) g^2;
+// p -= lr / (1 - b1^t) * m / (sqrt(v) / sqrt(1 - b2^t) + eps), with g += weight_decay * p first.
+// omb1 / omb2 = 1 - b1 / 1 - b2 rounded once from double, as torch rounds its `1 - beta` scalars: 1 - 0.999f would
+// be 1.3e-5 off 0.001, and exp_avg_sq with it.
+__global__ void adam_kernel(AdamTensors T, float lr, float b1, float omb1, float b2, float omb2, float eps,
+                            float weight_decay, float bc1, float bc2_sqrt) {
   const int t = blockIdx.y;
   if (t >= T.count) return;
   float* p = T.p[t];
@@ -106,8 +109,9 @@ __global__ void adam_kernel(AdamTensors T, float lr, float b1, float b2, float e
     float gi = g[i];
     const float pi = p[i];
     if (weight_decay != 0.f) gi = fmaf(weight_decay, pi, gi);
-    const float mi = fmaf(b1, m[i], (1.0f - b1) * gi);
-    const float vi = fmaf(b2, v[i], (1.0f - b2) * gi * gi);
+    // exp_avg.lerp_(g, 1 - b1) in torch's form, so that an infinite moment meets the next gradient as torch's does
+    const float mi = omb1 < 0.5f ? fmaf(omb1, gi - m[i], m[i]) : gi - (gi - m[i]) * (1.0f - omb1);
+    const float vi = fmaf(b2, v[i], omb2 * gi * gi);
     m[i] = mi;
     v[i] = vi;
     p[i] = pi - step * (mi / (sqrtf(vi) / bc2_sqrt + eps));
@@ -136,30 +140,36 @@ extern "C" int32_t neddf_render_loss(const float* d_color, const float* d_color_
 
 extern "C" int32_t neddf_field_adam_step(neddf_field_t* f, float* const* d_params, const float* const* d_grads,
                                          float* const* d_exp_avg, float* const* d_exp_avg_sq, const int64_t* h_numel,
-                                         int32_t n_tensors, float lr, float beta1, float beta2, float eps,
+                                         int32_t n_tensors, float lr, double beta1, double beta2, float eps,
                                          float weight_decay, int64_t step, void* stream) {
   if (!d_params || !d_grads || !d_exp_avg || !d_exp_avg_sq || !h_numel) return fail(NEDDF_E_INVALID, "neddf_field_adam_step: NULL argument");
   if (n_tensors < 1 || n_tensors > 64 || step < 1) return fail(NEDDF_E_INVALID, "neddf_field_adam_step: bad n_tensors / step");
+  // every argument is checked before the first launch: a refused call leaves every tensor as it was
+  for (int i = 0; i < n_tensors; ++i) {
+    // an empty tensor's storage may be NULL (torch's is); a field's layers are never empty
+    if ((h_numel[i] > 0 || f) && (!d_params[i] || !d_grads[i] || !d_exp_avg[i] || !d_exp_avg_sq[i]))
+      return fail(NEDDF_E_INVALID, "neddf_field_adam_step: NULL tensor " + std::to_string(i));
+    if (h_numel[i] < 0) return fail(NEDDF_E_INVALID, "neddf_field_adam_step: negative numel of tensor " + std::to_string(i));
+  }
+  if (f && n_tensors != 2 * f->n_layers) return fail(NEDDF_E_INVALID, "neddf_field_adam_step: a field needs weight, bias per layer");
   cudaStream_t s = (cudaStream_t)stream;
-  const float bc1 = (float)(1.0 - pow((double)beta1, (double)step));
-  const float bc2_sqrt = (float)sqrt(1.0 - pow((double)beta2, (double)step));
+  const float bc1 = (float)(1.0 - pow(beta1, (double)step));
+  const float bc2_sqrt = (float)sqrt(1.0 - pow(beta2, (double)step));
   for (int base = 0; base < n_tensors; base += 32) {
     AdamTensors T;
     T.count = n_tensors - base < 32 ? n_tensors - base : 32;
     for (int i = 0; i < T.count; ++i) {
-      if (!d_params[base + i] || !d_grads[base + i] || !d_exp_avg[base + i] || !d_exp_avg_sq[base + i])
-        return fail(NEDDF_E_INVALID, "neddf_field_adam_step: NULL tensor");
       T.p[i] = d_params[base + i];
       T.g[i] = d_grads[base + i];
       T.m[i] = d_exp_avg[base + i];
       T.v[i] = d_exp_avg_sq[base + i];
       T.n[i] = h_numel[base + i];
     }
-    adam_kernel<<<dim3(32, T.count), 256, 0, s>>>(T, lr, beta1, beta2, eps, weight_decay, bc1, bc2_sqrt);
+    adam_kernel<<<dim3(32, T.count), 256, 0, s>>>(T, lr, (float)beta1, (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2),
+                                                  eps, weight_decay, bc1, bc2_sqrt);
     NEDDF_LAUNCH_CHECK();
   }
   if (f) {  // re-pack the kernel-layout weights from the updated parameters (2 tensors per layer, reference order)
-    if (n_tensors != 2 * f->n_layers) return fail(NEDDF_E_INVALID, "neddf_field_adam_step: a field needs weight, bias per layer");
     std::vector<const float*> w(f->n_layers), b(f->n_layers);
     for (int i = 0; i < f->n_layers; ++i) {
       w[i] = d_params[2 * i];

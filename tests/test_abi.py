@@ -32,7 +32,7 @@ def test_python_binding_covers_header(repo_root, built):
     from neddf_b200 import _lib as L
     assert L.exported_symbols() == _declared(repo_root)
     lib = L.lib()
-    assert lib.neddf_abi_version() == 2
+    assert lib.neddf_abi_version() == 3
     assert lib.neddf_launch_count() == 0
 
 
