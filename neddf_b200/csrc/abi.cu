@@ -332,20 +332,47 @@ static int32_t dispatch(const neddf_field* f, FieldParams& p, int32_t flags, int
   return fail(NEDDF_E_INVALID, "unknown engine id");
 }
 
+// The checks of the entry points on explicit samples, in this order: field, weights, n (empty_ok: n == 0 is an empty
+// launch, p.n == 0 on return), input pointers, state.
+static int32_t fill_samples(const neddf_field* f, const neddf_field_state_t* st, FieldParams& p, const float* d_pos,
+                            const float* d_dir, const float* d_var, int64_t n, bool empty_ok, const char* who) {
+  if (!f) return fail(NEDDF_E_INVALID, std::string(who) + ": field is NULL");
+  if (!f->weights_set) return fail(NEDDF_E_INVALID, std::string(who) + ": weights were never set");
+  if (empty_ok ? n < 0 : n <= 0) return fail(NEDDF_E_INVALID, std::string(who) + (empty_ok ? ": n < 0" : ": n <= 0"));
+  p = f->proto;
+  if (n == 0) return NEDDF_OK;
+  if (!d_pos || !d_dir || !d_var) return fail(NEDDF_E_INVALID, std::string(who) + ": NULL input pointer");
+  set_samples(p, n, d_pos, d_dir, d_var);
+  return fill_state(f, st, p);
+}
+
+// The checks of the entry points on rays, in this order: field, weights, sizes (seg: and its bounds), sampling type
+// (check_field_rays; empty_ok: n_rays == 0 is an empty launch, p.n == 0 on return), input pointers (seg: and
+// the outputs d_density, d_color), the ray list with its count (seg), state.
+static int32_t fill_rays(const neddf_field* f, const neddf_field_state_t* st, FieldParams& p, const float* d_ray_dir,
+                         const float* d_ray_orig, const float* d_dists, int64_t n_rays, int32_t n_edges,
+                         int32_t sampling_type, float ray_radius, bool empty_ok, const char* who,
+                         const Segment* seg = nullptr, const float* d_density = nullptr, const float* d_color = nullptr) {
+  if (!f) return fail(NEDDF_E_INVALID, std::string(who) + ": field is NULL");
+  if (!f->weights_set) return fail(NEDDF_E_INVALID, std::string(who) + ": weights were never set");
+  if (int32_t rc = check_field_rays(who, n_rays, n_edges, sampling_type, empty_ok, seg)) return rc;
+  p = f->proto;
+  if (n_rays == 0) return NEDDF_OK;
+  if (!d_ray_dir || !d_ray_orig || !d_dists || (seg && (!d_density || !d_color)))
+    return fail(NEDDF_E_INVALID, std::string(who) + (seg ? ": NULL pointer" : ": NULL input pointer"));
+  if (seg && (seg->ray_index == nullptr) != (seg->n_active == nullptr))
+    return fail(NEDDF_E_INVALID, std::string(who) + ": d_ray_index and d_n_active go together");
+  set_rays(p, d_ray_dir, d_ray_orig, d_dists, n_rays, n_edges, sampling_type, ray_radius, seg ? *seg : Segment{});
+  return fill_state(f, st, p);
+}
+
 extern "C" int32_t neddf_field_forward(const neddf_field_t* f, const neddf_field_state_t* st, const float* d_pos,
                                        const float* d_dir, const float* d_var, int64_t n, float* d_distance,
                                        float* d_density, float* d_color, float* d_penalty, float* d_aux_grad,
                                        int32_t flags, int32_t engine, void* stream) {
-  if (!f) return fail(NEDDF_E_INVALID, "neddf_field_forward: field is NULL");
-  if (!f->weights_set) return fail(NEDDF_E_INVALID, "neddf_field_forward: weights were never set");
-  if (n < 0) return fail(NEDDF_E_INVALID, "neddf_field_forward: n < 0");
-  if (n == 0) return NEDDF_OK;
-  if (!d_pos || !d_dir || !d_var) return fail(NEDDF_E_INVALID, "neddf_field_forward: NULL input pointer");
-  FieldParams p = f->proto;
-  int32_t rc = fill_state(f, st, p);
-  if (rc != NEDDF_OK) return rc;
-  p.pos = d_pos; p.dir = d_dir; p.var = d_var;
-  p.n = n;
+  FieldParams p;
+  int32_t rc = fill_samples(f, st, p, d_pos, d_dir, d_var, n, /*empty_ok=*/true, "neddf_field_forward");
+  if (rc != NEDDF_OK || p.n == 0) return rc;
   p.distance = d_distance; p.density = d_density; p.color = d_color; p.penalty = d_penalty; p.aux_grad = d_aux_grad;
   return dispatch(f, p, flags, engine, (cudaStream_t)stream);
 }
@@ -355,21 +382,10 @@ extern "C" int32_t neddf_field_forward_rays(const neddf_field_t* f, const neddf_
                                             int64_t n_rays, int32_t n_edges, int32_t sampling_type, float ray_radius,
                                             float* d_distance, float* d_density, float* d_color, float* d_penalty,
                                             float* d_aux_grad, int32_t flags, int32_t engine, void* stream) {
-  if (!f) return fail(NEDDF_E_INVALID, "neddf_field_forward_rays: field is NULL");
-  if (!f->weights_set) return fail(NEDDF_E_INVALID, "neddf_field_forward_rays: weights were never set");
-  if (n_rays < 0 || n_edges < 1) return fail(NEDDF_E_INVALID, "neddf_field_forward_rays: bad sizes");
-  if (sampling_type != NEDDF_SAMPLING_POINT && sampling_type != NEDDF_SAMPLING_CONE)
-    return fail(NEDDF_E_INVALID, "neddf_field_forward_rays: unknown sampling type");
-  if (sampling_type == NEDDF_SAMPLING_CONE && n_edges < 2)
-    return fail(NEDDF_E_INVALID, "neddf_field_forward_rays: cone sampling needs >= 2 edges");
-  if (n_rays == 0) return NEDDF_OK;
-  if (!d_ray_dir || !d_ray_orig || !d_dists) return fail(NEDDF_E_INVALID, "neddf_field_forward_rays: NULL input pointer");
-  FieldParams p = f->proto;
-  int32_t rc = fill_state(f, st, p);
-  if (rc != NEDDF_OK) return rc;
-  p.ray_dir = d_ray_dir; p.ray_orig = d_ray_orig; p.dists = d_dists;
-  p.n_edges = n_edges; p.sampling_type = sampling_type; p.ray_radius = ray_radius;
-  p.n = n_rays * (int64_t)n_edges;
+  FieldParams p;
+  int32_t rc = fill_rays(f, st, p, d_ray_dir, d_ray_orig, d_dists, n_rays, n_edges, sampling_type, ray_radius,
+                         /*empty_ok=*/true, "neddf_field_forward_rays");
+  if (rc != NEDDF_OK || p.n == 0) return rc;
   p.distance = d_distance; p.density = d_density; p.color = d_color; p.penalty = d_penalty; p.aux_grad = d_aux_grad;
   return dispatch(f, p, flags, engine, (cudaStream_t)stream);
 }
@@ -383,26 +399,11 @@ extern "C" int32_t neddf_field_forward_rays_segment(const neddf_field_t* f, cons
                                                     float ray_radius, int32_t edge0, int32_t seg_len,
                                                     const int32_t* d_ray_index, const int32_t* d_n_active,
                                                     float* d_density, float* d_color, int32_t engine, void* stream) {
-  if (!f) return fail(NEDDF_E_INVALID, "neddf_field_forward_rays_segment: field is NULL");
-  if (!f->weights_set) return fail(NEDDF_E_INVALID, "neddf_field_forward_rays_segment: weights were never set");
-  if (n_rays < 0 || n_edges < 1 || edge0 < 0 || seg_len < 1 || edge0 + seg_len > n_edges)
-    return fail(NEDDF_E_INVALID, "neddf_field_forward_rays_segment: bad sizes");
-  if (sampling_type != NEDDF_SAMPLING_POINT && sampling_type != NEDDF_SAMPLING_CONE)
-    return fail(NEDDF_E_INVALID, "neddf_field_forward_rays_segment: unknown sampling type");
-  if (sampling_type == NEDDF_SAMPLING_CONE && n_edges < 2)
-    return fail(NEDDF_E_INVALID, "neddf_field_forward_rays_segment: cone sampling needs >= 2 edges");
-  if (n_rays == 0) return NEDDF_OK;
-  if (!d_ray_dir || !d_ray_orig || !d_dists || !d_density || !d_color)
-    return fail(NEDDF_E_INVALID, "neddf_field_forward_rays_segment: NULL pointer");
-  if ((d_ray_index == nullptr) != (d_n_active == nullptr))
-    return fail(NEDDF_E_INVALID, "neddf_field_forward_rays_segment: d_ray_index and d_n_active go together");
-  FieldParams p = f->proto;
-  int32_t rc = fill_state(f, st, p);
-  if (rc != NEDDF_OK) return rc;
-  p.ray_dir = d_ray_dir; p.ray_orig = d_ray_orig; p.dists = d_dists;
-  p.n_edges = n_edges; p.sampling_type = sampling_type; p.ray_radius = ray_radius;
-  p.n = n_rays * (int64_t)seg_len;  // upper bound: sizes the grid; the kernel reads *d_n_active
-  p.seg_len = seg_len; p.seg_edge0 = edge0; p.ray_index = d_ray_index; p.n_active = d_n_active;
+  const Segment seg{seg_len, edge0, d_ray_index, d_n_active};
+  FieldParams p;
+  int32_t rc = fill_rays(f, st, p, d_ray_dir, d_ray_orig, d_dists, n_rays, n_edges, sampling_type, ray_radius,
+                         /*empty_ok=*/true, "neddf_field_forward_rays_segment", &seg, d_density, d_color);
+  if (rc != NEDDF_OK || p.n == 0) return rc;
   p.density = d_density; p.color = d_color;
   return dispatch(f, p, NEDDF_OUT_EVAL, engine, (cudaStream_t)stream);
 }
@@ -410,23 +411,11 @@ extern "C" int32_t neddf_field_forward_rays_segment(const neddf_field_t* f, cons
 // ---------------------------------------------------------------------------------------------
 // training path
 // ---------------------------------------------------------------------------------------------
-static int32_t fill_rays(const neddf_field* f, const neddf_field_state_t* st, FieldParams& p, const float* d_ray_dir,
-                         const float* d_ray_orig, const float* d_dists, int64_t n_rays, int32_t n_edges,
-                         int32_t sampling_type, float ray_radius, const char* who) {
-  if (!f) return fail(NEDDF_E_INVALID, std::string(who) + ": field is NULL");
-  if (!f->weights_set) return fail(NEDDF_E_INVALID, std::string(who) + ": weights were never set");
-  if (n_rays <= 0 || n_edges < 1) return fail(NEDDF_E_INVALID, std::string(who) + ": bad sizes");
-  if (sampling_type != NEDDF_SAMPLING_POINT && sampling_type != NEDDF_SAMPLING_CONE)
-    return fail(NEDDF_E_INVALID, std::string(who) + ": unknown sampling type");
-  if (sampling_type == NEDDF_SAMPLING_CONE && n_edges < 2) return fail(NEDDF_E_INVALID, std::string(who) + ": cone sampling needs >= 2 edges");
-  if (!d_ray_dir || !d_ray_orig || !d_dists) return fail(NEDDF_E_INVALID, std::string(who) + ": NULL input pointer");
-  p = f->proto;
-  int32_t rc = fill_state(f, st, p);
-  if (rc != NEDDF_OK) return rc;
-  p.ray_dir = d_ray_dir; p.ray_orig = d_ray_orig; p.dists = d_dists;
-  p.n_edges = n_edges; p.sampling_type = sampling_type; p.ray_radius = ray_radius;
-  p.n = n_rays * (int64_t)n_edges;
-  return NEDDF_OK;
+// the buffers of neddf_field_backward / _backward_samples (g_penalty may be NULL)
+static int32_t backward(const neddf_field* f, FieldParams& p, const BackwardIO& io, const char* who, void* stream) {
+  if (!io.save_pre || !io.g_density || !io.g_color || !io.post || !io.gpre || !io.ghead_da || !io.ghead_col || !io.xes || !io.xcol)
+    return fail(NEDDF_E_INVALID, std::string(who) + ": NULL buffer");
+  return launch_field_backward(f, p, io, (cudaStream_t)stream);
 }
 
 extern "C" int32_t neddf_field_forward_train(const neddf_field_t* f, const neddf_field_state_t* st,
@@ -436,7 +425,7 @@ extern "C" int32_t neddf_field_forward_train(const neddf_field_t* f, const neddf
                                              int32_t engine, void* stream) {
   FieldParams p;
   int32_t rc = fill_rays(f, st, p, d_ray_dir, d_ray_orig, d_dists, n_rays, n_edges, sampling_type, ray_radius,
-                         "neddf_field_forward_train");
+                         /*empty_ok=*/false, "neddf_field_forward_train");
   if (rc != NEDDF_OK) return rc;
   if (!d_save_pre) return fail(NEDDF_E_INVALID, "neddf_field_forward_train: d_save_pre is NULL");
   p.density = d_density; p.color = d_color; p.penalty = d_penalty;
@@ -453,30 +442,10 @@ extern "C" int32_t neddf_field_backward(const neddf_field_t* f, const neddf_fiel
                                         float* d_xes, float* d_xcol, void* stream) {
   FieldParams p;
   int32_t rc = fill_rays(f, st, p, d_ray_dir, d_ray_orig, d_dists, n_rays, n_edges, sampling_type, ray_radius,
-                         "neddf_field_backward");
+                         /*empty_ok=*/false, "neddf_field_backward");
   if (rc != NEDDF_OK) return rc;
-  if (!d_save_pre || !g_density || !g_color || !d_post || !d_gpre || !d_ghead_da || !d_ghead_col || !d_xes || !d_xcol)
-    return fail(NEDDF_E_INVALID, "neddf_field_backward: NULL buffer");
-  BackwardIO io;
-  io.save_pre = d_save_pre;
-  io.g_density = g_density; io.g_color = g_color; io.g_penalty = g_penalty;
-  io.post = d_post; io.gpre = d_gpre; io.ghead_da = d_ghead_da; io.ghead_col = d_ghead_col;
-  io.xes = d_xes; io.xcol = d_xcol;
-  return launch_field_backward(f, p, io, (cudaStream_t)stream);
-}
-
-static int32_t fill_samples(const neddf_field* f, const neddf_field_state_t* st, FieldParams& p, const float* d_pos,
-                            const float* d_dir, const float* d_var, int64_t n, const char* who) {
-  if (!f) return fail(NEDDF_E_INVALID, std::string(who) + ": field is NULL");
-  if (!f->weights_set) return fail(NEDDF_E_INVALID, std::string(who) + ": weights were never set");
-  if (n <= 0) return fail(NEDDF_E_INVALID, std::string(who) + ": n <= 0");
-  if (!d_pos || !d_dir || !d_var) return fail(NEDDF_E_INVALID, std::string(who) + ": NULL input pointer");
-  p = f->proto;
-  int32_t rc = fill_state(f, st, p);
-  if (rc != NEDDF_OK) return rc;
-  p.pos = d_pos; p.dir = d_dir; p.var = d_var;
-  p.n = n;
-  return NEDDF_OK;
+  return backward(f, p, {d_save_pre, g_density, g_color, g_penalty, d_post, d_gpre, d_ghead_da, d_ghead_col, d_xes, d_xcol},
+                  "neddf_field_backward", stream);
 }
 
 extern "C" int32_t neddf_field_forward_train_samples(const neddf_field_t* f, const neddf_field_state_t* st,
@@ -485,7 +454,7 @@ extern "C" int32_t neddf_field_forward_train_samples(const neddf_field_t* f, con
                                                      float* d_penalty, float* d_aux_grad, float* d_save_pre,
                                                      int32_t engine, void* stream) {
   FieldParams p;
-  int32_t rc = fill_samples(f, st, p, d_pos, d_dir, d_var, n, "neddf_field_forward_train_samples");
+  int32_t rc = fill_samples(f, st, p, d_pos, d_dir, d_var, n, /*empty_ok=*/false, "neddf_field_forward_train_samples");
   if (rc != NEDDF_OK) return rc;
   if (!d_save_pre) return fail(NEDDF_E_INVALID, "neddf_field_forward_train_samples: d_save_pre is NULL");
   p.distance = d_distance; p.density = d_density; p.color = d_color; p.penalty = d_penalty; p.aux_grad = d_aux_grad;
@@ -500,14 +469,8 @@ extern "C" int32_t neddf_field_backward_samples(const neddf_field_t* f, const ne
                                                 float* d_ghead_da, float* d_ghead_col, float* d_xes, float* d_xcol,
                                                 void* stream) {
   FieldParams p;
-  int32_t rc = fill_samples(f, st, p, d_pos, d_dir, d_var, n, "neddf_field_backward_samples");
+  int32_t rc = fill_samples(f, st, p, d_pos, d_dir, d_var, n, /*empty_ok=*/false, "neddf_field_backward_samples");
   if (rc != NEDDF_OK) return rc;
-  if (!d_save_pre || !g_density || !g_color || !d_post || !d_gpre || !d_ghead_da || !d_ghead_col || !d_xes || !d_xcol)
-    return fail(NEDDF_E_INVALID, "neddf_field_backward_samples: NULL buffer");
-  BackwardIO io;
-  io.save_pre = d_save_pre;
-  io.g_density = g_density; io.g_color = g_color; io.g_penalty = g_penalty;
-  io.post = d_post; io.gpre = d_gpre; io.ghead_da = d_ghead_da; io.ghead_col = d_ghead_col;
-  io.xes = d_xes; io.xcol = d_xcol;
-  return launch_field_backward(f, p, io, (cudaStream_t)stream);
+  return backward(f, p, {d_save_pre, g_density, g_color, g_penalty, d_post, d_gpre, d_ghead_da, d_ghead_col, d_xes, d_xcol},
+                  "neddf_field_backward_samples", stream);
 }

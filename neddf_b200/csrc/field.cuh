@@ -3,7 +3,7 @@
 
 #include <vector>
 
-#include "common.cuh"
+#include "samples.cuh"
 
 namespace neddf {
 
@@ -22,7 +22,7 @@ struct LayerDesc {
   int bias_off;    // offset (floats) into the packed bias array
 };
 
-struct FieldParams {
+struct FieldParams : Samples {  // the samples: where they come from, where their outputs go
   // network structure
   int n_ddf;  // hidden layers of the distance trunk (ddf_layer_count - 1)
   int n_col;  // hidden layers of the colour trunk   (col_layer_count - 1)
@@ -46,23 +46,6 @@ struct FieldParams {
   const float* w_head_da;  // [256][2]  (ddf_out, aux_out)
   const float* w_head_col; // [256][4]  (r,g,b,0)
   const float* b_head;     // [5] ddf, aux, r, g, b
-  // inputs: either Sampling tensors or rays + edge distances
-  const float* pos;
-  const float* dir;
-  const float* var;
-  const float* ray_dir;
-  const float* ray_orig;
-  const float* dists;
-  int n_edges;
-  int sampling_type;
-  float ray_radius;
-  int64_t n;  // samples (upper bound when n_active is given)
-  // segment view for early ray termination: samples [seg_edge0, seg_edge0 + seg_len) of the rays listed in
-  // ray_index[0 .. *n_active) (NULL = rays 0 .. n / seg_len); outputs land at [ray, edge] of the full arrays
-  int seg_len;     // 0 = whole rows
-  int seg_edge0;
-  const int32_t* ray_index;
-  const int32_t* n_active;  // device scalar, read by the kernel (no host synchronisation between segments)
   // outputs (any may be null)
   float* distance;
   float* density;
@@ -73,55 +56,6 @@ struct FieldParams {
   // then the 3 Jacobian rows), written by the fp32 engine when non-null
   float* save_pre;
 };
-
-// number of samples this launch processes / where sample n comes from and where its outputs go
-__device__ __forceinline__ int64_t field_total(const FieldParams& p) {
-  return (p.seg_len > 0 && p.n_active) ? (int64_t)(*p.n_active) * p.seg_len : p.n;
-}
-__device__ __forceinline__ void field_map(const FieldParams& p, int64_t n, int64_t& ray, int& j, int64_t& out) {
-  if (p.seg_len > 0) {
-    const int64_t r = n / p.seg_len;
-    j = p.seg_edge0 + (int)(n - r * p.seg_len);
-    ray = p.ray_index ? (int64_t)p.ray_index[r] : r;
-    out = ray * p.n_edges + j;
-  } else {
-    ray = p.dists ? n / p.n_edges : 0;
-    j = p.dists ? (int)(n % p.n_edges) : 0;
-    out = n;
-  }
-}
-
-// Network inputs of sample n: explicit samples, or the cone / point of its ray interval (ray.py:88-194 fused).
-// Samples at or past n_total get a fixed harmless input (their outputs are never written).
-struct SampleIn {
-  float pos[3], dir[3], var[3];
-};
-__device__ __forceinline__ SampleIn sample_input(const FieldParams& p, int64_t n, int64_t n_total) {
-  SampleIn r = {{0.f, 0.f, 0.f}, {0.f, 0.f, 1.f}, {0.f, 0.f, 0.f}};
-  if (n < n_total) {
-    if (p.dists) {
-      int64_t b, out;
-      int j;
-      field_map(p, n, b, j, out);
-      const float* row = p.dists + b * p.n_edges;
-      float o[3];
-#pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        o[i] = p.ray_orig[3 * b + i];
-        r.dir[i] = p.ray_dir[3 * b + i];
-      }
-      sample_geometry(p.sampling_type, p.ray_radius, o, r.dir, row[j], far_edge(row, j, p.n_edges), r.pos, r.var);
-    } else {
-#pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        r.pos[i] = p.pos[3 * n + i];
-        r.dir[i] = p.dir[3 * n + i];
-        r.var[i] = p.var[3 * n + i];
-      }
-    }
-  }
-  return r;
-}
 
 // Buffers of the training backward (all device, fp32, row-major)
 struct BackwardIO {

@@ -202,7 +202,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_backward_kernel(const __gri
     };
 
     // ---------------- geometry, embeddings (inputs of the weight-gradient GEMMs) -------------------
-    if (cg == 0) sc.in = sample_input(p, my_n, p.n);
+    if (cg == 0) sc.in = sample_in(p, my_n, p.n);
     __syncthreads();
     if (valid) {
       const int half = 3 * p.embed_pos;

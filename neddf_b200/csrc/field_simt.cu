@@ -33,7 +33,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_simt_kernel(const __grid_co
   const int n_hidden = p.n_ddf + p.n_col;
   float* h = act + (size_t)p.off_h * kPitch;  // the hidden activations' rows of the K space
 
-  const int64_t n_total = field_total(p);
+  const int64_t n_total = sample_count(p);
   const int64_t n_tiles = (n_total + kTile - 1) / kTile;
   for (int i = tid; i < kWidth * 2; i += kThreads) head_da[i] = p.w_head_da[i];
   for (int i = tid; i < kWidth * 4; i += kThreads) head_col[i] = p.w_head_col[i];
@@ -45,7 +45,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_simt_kernel(const __grid_co
     const bool valid = my_n < n_total;
 
     // ---------------- prologue: geometry + embeddings -------------------------------------
-    if (cg == 0) scr[s_slot].in = sample_input(p, my_n, n_total);
+    if (cg == 0) scr[s_slot].in = sample_in(p, my_n, n_total);
     __syncthreads();
     {
       const SampleIn& in = scr[s_slot].in;
@@ -117,9 +117,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_simt_kernel(const __grid_co
       for (int c = 0; c < 3; ++c)
 #pragma unroll
         for (int i = 0; i < 3; ++i) colJ[i][c] = pc[1 + i][c];
-      int64_t ray_, on;  // where this sample's outputs go (segment view: [ray, edge] of the full arrays)
-      int j_;
-      field_map(p, my_n, ray_, j_, on);
+      const int64_t on = sample_out(p, my_n);
       if (p.distance) p.distance[on] = hd.distance;
       if (p.density) p.density[on] = hd.density;
       if (p.aux_grad) p.aux_grad[on] = hd.aux;

@@ -143,7 +143,7 @@ __device__ __forceinline__ void tma_bulk_g2s_pair(uint32_t dst_smem, const void*
 // ---------------------------------------------------------------------------------------------
 // geometry of the tile's samples -> scratch (one thread per sample)
 __device__ __forceinline__ void tile_geometry(const FieldParams& p, float (*geo)[12], int64_t n0, int s, int64_t n_total) {
-  const SampleIn in = sample_input(p, n0 + s, n_total);
+  const SampleIn in = sample_in(p, n0 + s, n_total);
 #pragma unroll
   for (int i = 0; i < 3; ++i) {
     geo[s][i] = in.pos[i];
@@ -240,7 +240,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
   const int n_hidden = p.n_ddf + p.n_col;
 
   // tiles: single CTAs take tiles blockIdx.x + t * gridDim.x; a pair takes tile pairs, CTA r the tile 2 pair + r
-  const int64_t n_total = field_total(p);
+  const int64_t n_total = sample_count(p);
   const int64_t n_tiles = (n_total + kTileS - 1) / kTileS;
   const uint32_t rank = PAIR ? cluster_ctarank() : 0;
   const int64_t unit = PAIR ? (int64_t)(blockIdx.x >> 1) : (int64_t)blockIdx.x;
@@ -465,9 +465,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
           }
           const int64_t n = n0 + hs;
           if (n < n_total) {
-            int64_t ray_, on;  // where this sample's outputs go (segment view: [ray, edge] of the full arrays)
-            int j_;
-            field_map(p, n, ray_, j_, on);
+            const int64_t on = sample_out(p, n);
             if (p.distance) p.distance[on] = head.distance;
             if (p.density) p.density[on] = head.density;
             if (p.aux_grad) p.aux_grad[on] = head.aux;
@@ -511,9 +509,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
           for (int c = 0; c < 3; ++c) pc[c] += __shfl_xor_sync(0xffffffffu, pc[c], 1);
           const int64_t n = tile_of(base + (row >> 5)) * kTileS + (row & 31);
           if (ck == 0 && (row >> 5) < gn && n < n_total && p.color) {
-            int64_t ray_, on;
-            int j_;
-            field_map(p, n, ray_, j_, on);
+            const int64_t on = sample_out(p, n);
 #pragma unroll
             for (int c = 0; c < 3; ++c) p.color[3 * on + c] = pc[c] + __ldg(p.b_head + 2 + c);
           }
@@ -544,9 +540,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
 #pragma unroll
               for (int j = 0; j < 3; ++j) colJ[j][c] = colv[1 + j][c];
             }
-            int64_t ray_, on;
-            int j_;
-            field_map(p, n, ray_, j_, on);
+            const int64_t on = sample_out(p, n);
             if (p.color) {
               p.color[3 * on + 0] = col[0];
               p.color[3 * on + 1] = col[1];

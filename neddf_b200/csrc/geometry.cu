@@ -1,6 +1,6 @@
 // K1: ray generation, stratified coarse edges, Sampling materialisation.
 // HBM-bound elementwise kernels; one thread per ray or per sample, coalesced.
-#include "common.cuh"
+#include "samples.cuh"
 
 namespace neddf {
 
@@ -66,27 +66,17 @@ __global__ void coarse_dists_kernel(const float* __restrict__ u, int64_t total, 
   dists[i] = NA(linspace_at(near_, far_, n_edges, j), NM(u[i], jitter));
 }
 
-__global__ void make_samples_kernel(const float* __restrict__ ray_dir, const float* __restrict__ ray_orig,
-                                    const float* __restrict__ dists, int64_t total, int n_edges,
-                                    int sampling_type, float ray_radius, float* __restrict__ pos,
-                                    float* __restrict__ dir, float* __restrict__ var) {
+// the fused sample geometry of the field kernels, materialised as a Sampling
+__global__ void make_samples_kernel(const __grid_constant__ Samples s, float* __restrict__ pos, float* __restrict__ dir,
+                                    float* __restrict__ var) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  int64_t b = i / n_edges;
-  int j = (int)(i % n_edges);
-  const float* row = dists + b * n_edges;
-  float o[3], d[3], p[3], v[3];
+  if (i >= s.n) return;
+  const SampleIn in = ray_sample_in(s, i);
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
-    o[k] = ray_orig[3 * b + k];
-    d[k] = ray_dir[3 * b + k];
-  }
-  sample_geometry(sampling_type, ray_radius, o, d, row[j], far_edge(row, j, n_edges), p, v);
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    pos[3 * i + k] = p[k];
-    dir[3 * i + k] = d[k];
-    var[3 * i + k] = v[k];
+    pos[3 * i + k] = in.pos[k];
+    dir[3 * i + k] = in.dir[k];
+    var[3 * i + k] = in.var[k];
   }
 }
 
@@ -173,19 +163,15 @@ extern "C" int32_t neddf_coarse_dists(const float* d_u, int64_t n_rays, int32_t 
 extern "C" int32_t neddf_make_samples(const float* d_ray_dir, const float* d_ray_orig, const float* d_dists,
                                       int64_t n_rays, int32_t n_edges, int32_t sampling_type, float ray_radius,
                                       float* d_pos, float* d_dir, float* d_var, void* stream) {
-  if (n_rays < 0 || n_edges < 1) return fail(NEDDF_E_INVALID, "neddf_make_samples: bad sizes");
-  if (sampling_type != NEDDF_SAMPLING_POINT && sampling_type != NEDDF_SAMPLING_CONE)
-    return fail(NEDDF_E_INVALID, "neddf_make_samples: unknown sampling type");
-  if (sampling_type == NEDDF_SAMPLING_CONE && n_edges < 2)
-    return fail(NEDDF_E_INVALID, "neddf_make_samples: cone sampling needs >= 2 edges");
+  if (int32_t rc = check_field_rays("neddf_make_samples", n_rays, n_edges, sampling_type, /*empty_ok=*/true)) return rc;
   if (n_rays == 0) return NEDDF_OK;
   if (!d_ray_dir || !d_ray_orig || !d_dists || !d_pos || !d_dir || !d_var)
     return fail(NEDDF_E_INVALID, "neddf_make_samples: null device pointer");
-  int64_t total = n_rays * n_edges;
+  Samples smp;
+  set_rays(smp, d_ray_dir, d_ray_orig, d_dists, n_rays, n_edges, sampling_type, ray_radius);
   int threads = 256;
-  int64_t blocks = (total + threads - 1) / threads;
-  make_samples_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(
-      d_ray_dir, d_ray_orig, d_dists, total, n_edges, sampling_type, ray_radius, d_pos, d_dir, d_var);
+  int64_t blocks = (smp.n + threads - 1) / threads;
+  make_samples_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(smp, d_pos, d_dir, d_var);
   NEDDF_LAUNCH_CHECK();
   return NEDDF_OK;
 }

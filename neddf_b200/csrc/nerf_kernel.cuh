@@ -51,7 +51,7 @@ struct Layer {
   int wt_off, kt_pad;  // training only: transposed pack [kt_pad (output channels)][256 (input channels of the h part)]
 };
 
-struct Params {
+struct Params : Samples {
   // network
   int n_layers;  // hidden layers; layer n_layers is the colour branch's first layer (128 outputs)
   Layer layer[kMaxLayers];
@@ -60,13 +60,6 @@ struct Params {
   int density_act;
   int w_density_off, w_col2_off;  // [256] + bias ; [3][128] + 3 biases
   float lowpass[16];
-  // inputs: explicit samples or rays + edges
-  int64_t n;
-  const float *pos, *dir, *var;
-  const float *ray_dir, *ray_orig, *dists;
-  int n_edges, sampling_type;
-  float ray_radius;
-  simt::Segment seg;  // early ray termination (zero: whole rows); n is then the grid's bound rays x seg.len
   // outputs ([n], [n, 3])
   float* density;
   float* color;
@@ -104,7 +97,7 @@ __device__ __forceinline__ void layer_gemm(Ctx& cx, const Params& P, const Layer
   simt::gemm(cx, P.w + L.w_off, L.k_pad, seg_ptr(smem, L.seg_a), L.n_a, seg_ptr(smem, L.seg_b), L.n_b, smem + kOffW, acc);
 }
 
-// Geometry of tile n0's samples (one thread per sample; sample n of P.seg's view), then the embeddings E and D
+// Geometry of tile n0's samples (one thread per sample), then the embeddings E and D
 // (nerf.py:133-142, four threads per sample).  Exit: behind a barrier.
 template <class Ctx>
 __device__ __forceinline__ void prologue(Ctx& cx, const Params& P, float* smem, int64_t n0) {
@@ -113,35 +106,12 @@ __device__ __forceinline__ void prologue(Ctx& cx, const Params& P, float* smem, 
   float* geo = smem + kOffGeo;
   const int tid = cx.tid;
   if (tid < kT) {
-    float pos[3] = {0.f, 0.f, 0.f}, dir[3] = {0.f, 0.f, 1.f}, var[3] = {0.f, 0.f, 0.f};
-    const int64_t n = n0 + tid;
-    if (n < simt::seg_total(P.seg, P.n)) {
-      if (P.dists) {
-        int64_t b;
-        int j;
-        simt::seg_ray_edge(P.seg, P.n_edges, n, b, j);
-        const float* row = P.dists + b * P.n_edges;
-        float o[3];
-#pragma unroll
-        for (int i = 0; i < 3; ++i) {
-          o[i] = P.ray_orig[3 * b + i];
-          dir[i] = P.ray_dir[3 * b + i];
-        }
-        sample_geometry(P.sampling_type, P.ray_radius, o, dir, row[j], far_edge(row, j, P.n_edges), pos, var);
-      } else {
-#pragma unroll
-        for (int i = 0; i < 3; ++i) {
-          pos[i] = P.pos[3 * n + i];
-          dir[i] = P.dir[3 * n + i];
-          var[i] = P.var[3 * n + i];
-        }
-      }
-    }
+    const SampleIn in = sample_in(P, n0 + tid, sample_count(P));
 #pragma unroll
     for (int i = 0; i < 3; ++i) {
-      geo[tid * 9 + i] = pos[i];
-      geo[tid * 9 + 3 + i] = dir[i];
-      geo[tid * 9 + 6 + i] = var[i];
+      geo[tid * 9 + i] = in.pos[i];
+      geo[tid * 9 + 3 + i] = in.dir[i];
+      geo[tid * 9 + 6 + i] = in.var[i];
     }
   }
   cx.sync();
@@ -178,7 +148,7 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
   float* H = smem + kOffH;
   const int tid = cx.tid;
   const int cg = tid & 15, sg = tid >> 4;
-  const int64_t n_total = simt::seg_total(P.seg, P.n);
+  const int64_t n_total = sample_count(P);
   const int64_t n_tiles = (n_total + kT - 1) / kT;
   float acc[4][4][4];
 
@@ -190,7 +160,7 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
         // density head on the trunk's features, before the colour branch overwrites H
         const int64_t n = n0 + tid;
         const float zd = density_pre(P, H, tid);
-        if (n < n_total) P.density[simt::seg_out(P.seg, P.n_edges, n)] = density_act(P.density_act, zd);
+        if (n < n_total) P.density[sample_out(P, n)] = density_act(P.density_act, zd);
       }
       // (no barrier needed: the layer below starts by reading H and only writes it after its own barriers)
       const Layer& L = P.layer[l];
@@ -225,7 +195,7 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
         o[c] = a;
       }
       if (n < n_total) {
-        const int64_t on = simt::seg_out(P.seg, P.n_edges, n);
+        const int64_t on = sample_out(P, n);
         P.color[3 * on + 0] = o[0];
         P.color[3 * on + 1] = o[1];
         P.color[3 * on + 2] = o[2];

@@ -72,8 +72,7 @@ extern "C" int32_t neddf_nerf_forward(const neddf_nerf_t* h, const float* lowpas
                                       const float* d_var, int64_t n, float* d_density, float* d_color, void* stream) {
   if (!h || !d_pos || !d_dir || !d_var || !d_density || !d_color) return fail(NEDDF_E_INVALID, "neddf_nerf_forward: null argument");
   nerf::Params P = h->proto;
-  P.n = n;
-  P.pos = d_pos; P.dir = d_dir; P.var = d_var;
+  set_samples(P, n, d_pos, d_dir, d_var);
   P.density = d_density; P.color = d_color;
   return nerf_launch(h, P, lowpass, stream);
 }
@@ -84,9 +83,7 @@ extern "C" int32_t neddf_nerf_forward_rays(const neddf_nerf_t* h, const float* l
   if (!h || !d_ray_dir || !d_ray_orig || !d_dists || !d_density || !d_color) return fail(NEDDF_E_INVALID, "neddf_nerf_forward_rays: null argument");
   if (int32_t rc = simt::check_rays("neddf_nerf_forward_rays", n_edges, sampling_type)) return rc;
   nerf::Params P = h->proto;
-  P.n = n_rays * n_edges;
-  P.ray_dir = d_ray_dir; P.ray_orig = d_ray_orig; P.dists = d_dists;
-  P.n_edges = n_edges; P.sampling_type = sampling_type; P.ray_radius = ray_radius;
+  set_rays(P, d_ray_dir, d_ray_orig, d_dists, n_rays, n_edges, sampling_type, ray_radius);
   P.density = d_density; P.color = d_color;
   return nerf_launch(h, P, lowpass, stream);
 }
@@ -99,13 +96,10 @@ extern "C" int32_t neddf_nerf_forward_rays_segment(const neddf_nerf_t* h, const 
   const char* who = "neddf_nerf_forward_rays_segment";
   if (!h || !d_ray_dir || !d_ray_orig || !d_dists || !d_density || !d_color) return fail(NEDDF_E_INVALID, std::string(who) + ": null argument");
   if (int32_t rc = simt::check_rays(who, n_edges, sampling_type)) return rc;
-  simt::Segment seg;
-  if (int32_t rc = simt::check_segment(who, n_edges, edge0, seg_len, d_ray_index, d_n_active, seg)) return rc;
+  const Segment seg{seg_len, edge0, d_ray_index, d_n_active};
+  if (int32_t rc = check_segment(who, n_edges, seg)) return rc;
   nerf::Params P = h->proto;
-  P.seg = seg;
-  P.n = n_rays * seg_len;  // bound of the grid; the kernel reads *d_n_active
-  P.ray_dir = d_ray_dir; P.ray_orig = d_ray_orig; P.dists = d_dists;
-  P.n_edges = n_edges; P.sampling_type = sampling_type; P.ray_radius = ray_radius;
+  set_rays(P, d_ray_dir, d_ray_orig, d_dists, n_rays, n_edges, sampling_type, ray_radius, seg);
   P.density = d_density; P.color = d_color;
   return nerf_launch(h, P, lowpass, stream);
 }

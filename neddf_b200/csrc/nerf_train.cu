@@ -53,8 +53,7 @@ extern "C" int32_t neddf_nerf_train_backward(const neddf_nerf_train_t* h, const 
                                              float* d_g, float* d_e, float* d_d, float* d_c1, float* d_gc1, float* d_gzd, void* stream) {
   if (!h || !d_pos || !d_dir || !d_var) return fail(NEDDF_E_INVALID, "neddf_nerf_train_backward: null argument");
   nerft::Params P = h->proto;
-  P.n = n;
-  P.pos = d_pos; P.dir = d_dir; P.var = d_var;
+  set_samples(P, n, d_pos, d_dir, d_var);
   return nerf_train_launch(h, P, lowpass, d_g_density, d_g_color, d_x, d_g, d_e, d_d, d_c1, d_gc1, d_gzd, stream);
 }
 
@@ -66,8 +65,6 @@ extern "C" int32_t neddf_nerf_train_backward_rays(const neddf_nerf_train_t* h, c
   if (!h || !d_ray_dir || !d_ray_orig || !d_dists) return fail(NEDDF_E_INVALID, "neddf_nerf_train_backward_rays: null argument");
   if (int32_t rc = simt::check_rays("neddf_nerf_train_backward_rays", n_edges, sampling_type)) return rc;
   nerft::Params P = h->proto;
-  P.n = n_rays * n_edges;
-  P.ray_dir = d_ray_dir; P.ray_orig = d_ray_orig; P.dists = d_dists;
-  P.n_edges = n_edges; P.sampling_type = sampling_type; P.ray_radius = ray_radius;
+  set_rays(P, d_ray_dir, d_ray_orig, d_dists, n_rays, n_edges, sampling_type, ray_radius);
   return nerf_train_launch(h, P, lowpass, d_g_density, d_g_color, d_x, d_g, d_e, d_d, d_c1, d_gc1, d_gzd, stream);
 }

@@ -56,7 +56,7 @@ struct Layer {
   int seg_b, n_b;  // second one (kSegNone: none)
 };
 
-struct Params {
+struct Params : Samples {  // var unused
   // network
   int n_sdf, n_col;
   Layer lsdf[kMaxSdf];
@@ -66,13 +66,6 @@ struct Params {
   int embed_pos, embed_dir;
   int act;       // NEDDF_ACT_RELU | NEDDF_ACT_TANHEXP
   const float* w;
-  // inputs: explicit samples or rays + edges
-  int64_t n;
-  const float *pos, *dir;
-  const float *ray_dir, *ray_orig, *dists;
-  int n_edges, sampling_type;
-  float ray_radius;
-  simt::Segment seg;  // early ray termination (zero: whole rows); n is then the grid's bound rays x seg.len
   // outputs ([n], [n], [n,3], optional [n,3]; sdf optional too, NULL in segment launches)
   float* sdf;
   float* density;
@@ -135,7 +128,7 @@ __device__ __forceinline__ void layer_gemm(Ctx& cx, const Params& P, const Layer
   simt::gemm(cx, P.w + L.w_off, L.k_pad, A, L.n_a, B, L.n_b, smem + kOffW, acc);
 }
 
-// Geometry of tile n0's samples (one thread per sample; sample n of P.seg's view) into geo and rows 0..2 of X
+// Geometry of tile n0's samples (one thread per sample) into geo and rows 0..2 of X
 // (position, neus.py:145), then the direction embedding into X (neus.py:120, four threads per sample).  Exit: NOT
 // behind a barrier - X is first read by the colour trunk, behind the barriers of the SDF trunk.
 template <class Ctx>
@@ -144,34 +137,12 @@ __device__ __forceinline__ void prologue(Ctx& cx, const Params& P, float* smem, 
   float* geo = smem + kOffGeo;
   const int tid = cx.tid;
   if (tid < kT) {
-    float pos[3] = {0.f, 0.f, 0.f}, dir[3] = {0.f, 0.f, 1.f}, var[3];
-    const int64_t n = n0 + tid;
-    if (n < simt::seg_total(P.seg, P.n)) {
-      if (P.dists) {
-        int64_t b;
-        int j;
-        simt::seg_ray_edge(P.seg, P.n_edges, n, b, j);
-        const float* row = P.dists + b * P.n_edges;
-        float o[3];
-#pragma unroll
-        for (int i = 0; i < 3; ++i) {
-          o[i] = P.ray_orig[3 * b + i];
-          dir[i] = P.ray_dir[3 * b + i];
-        }
-        sample_geometry(P.sampling_type, P.ray_radius, o, dir, row[j], far_edge(row, j, P.n_edges), pos, var);
-      } else {
-#pragma unroll
-        for (int i = 0; i < 3; ++i) {
-          pos[i] = P.pos[3 * n + i];
-          dir[i] = P.dir[3 * n + i];
-        }
-      }
-    }
+    const SampleIn in = sample_in(P, n0 + tid, sample_count(P));
 #pragma unroll
     for (int i = 0; i < 3; ++i) {
-      geo[tid * 6 + i] = pos[i];
-      geo[tid * 6 + 3 + i] = dir[i];
-      X[i * kT + tid] = pos[i];
+      geo[tid * 6 + i] = in.pos[i];
+      geo[tid * 6 + 3 + i] = in.dir[i];
+      X[i * kT + tid] = in.pos[i];
     }
   }
   cx.sync();
@@ -251,7 +222,7 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
   float* sdfv = smem + kOffSdf;
   const int tid = cx.tid;
   const int cg = tid & 15, sg = tid >> 4;
-  const int64_t n_total = simt::seg_total(P.seg, P.n);
+  const int64_t n_total = sample_count(P);
   const int64_t n_tiles = (n_total + kT - 1) / kT;
   const int x_normal = 3 + 2 * (3 * P.embed_dir);  // first normal row of X
   float acc[4][4][4];
@@ -283,7 +254,7 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
     if (tid < kT) {
       const int64_t n = n0 + tid;
       if (n < n_total) {
-        const int64_t on = simt::seg_out(P.seg, P.n_edges, n);
+        const int64_t on = sample_out(P, n);
         const float s = sdfv[tid];
         if (P.sdf) P.sdf[on] = s;
         P.density[on] = sdf_density(s, NEUS_LDG(P.w + P.var_off));
@@ -325,7 +296,7 @@ __device__ __forceinline__ void tile_program(Ctx& cx, const Params& P, float* sm
         act_fdd(P.act, colour_head_pre(P, H, tid, c), o[c], d1, d2);
       }
       if (n < n_total) {
-        const int64_t on = simt::seg_out(P.seg, P.n_edges, n);
+        const int64_t on = sample_out(P, n);
         P.color[3 * on + 0] = o[0];
         P.color[3 * on + 1] = o[1];
         P.color[3 * on + 2] = o[2];

@@ -59,8 +59,7 @@ extern "C" int32_t neddf_neus_train_backward(const neddf_neus_train_t* h, const 
                                              const float* d_g_normal, float* const* d_bufs, void* stream) {
   if (!h || !d_pos || !d_dir || !d_bufs) return fail(NEDDF_E_INVALID, "neddf_neus_train_backward: null argument");
   neust::Params T = h->proto;
-  T.f.n = n;
-  T.f.pos = d_pos; T.f.dir = d_dir;
+  set_samples(T.f, n, d_pos, d_dir, nullptr);
   return neus_train_launch(h, T, d_g_sdf, d_g_density, d_g_color, d_g_normal, d_bufs, stream);
 }
 
@@ -71,8 +70,6 @@ extern "C" int32_t neddf_neus_train_backward_rays(const neddf_neus_train_t* h, c
   if (!h || !d_ray_dir || !d_ray_orig || !d_dists || !d_bufs) return fail(NEDDF_E_INVALID, "neddf_neus_train_backward_rays: null argument");
   if (int32_t rc = simt::check_rays("neddf_neus_train_backward_rays", n_edges, sampling_type)) return rc;
   neust::Params T = h->proto;
-  T.f.n = n_rays * n_edges;
-  T.f.ray_dir = d_ray_dir; T.f.ray_orig = d_ray_orig; T.f.dists = d_dists;
-  T.f.n_edges = n_edges; T.f.sampling_type = sampling_type; T.f.ray_radius = ray_radius;
+  set_rays(T.f, d_ray_dir, d_ray_orig, d_dists, n_rays, n_edges, sampling_type, ray_radius);
   return neus_train_launch(h, T, d_g_sdf, d_g_density, d_g_color, d_g_normal, d_bufs, stream);
 }

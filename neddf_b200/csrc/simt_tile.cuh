@@ -11,7 +11,7 @@
 // emul::HostCtx (tests/emul/emul_common.h) when g++ compiles them into the host emulations of the CPU tests.
 #pragma once
 
-#include "common.cuh"
+#include "samples.cuh"
 
 #ifdef __CUDACC__
 #include <algorithm>
@@ -25,6 +25,7 @@ constexpr int kT = 64;        // samples per tile
 constexpr int kW = 256;       // layer width (fixed)
 constexpr int kChunk = 16;    // weight rows per shared-memory chunk
 constexpr int kThreads = 256;
+using neddf::Segment;  // the early-termination view as the host emulations (tests/emul) name it
 
 #ifdef __CUDACC__
 struct CudaCtx {
@@ -96,40 +97,6 @@ __device__ __forceinline__ void gemm(Ctx& cx, const float* wl, int k_pad, const 
   }
 }
 
-// Segment view of a _rays launch for early ray termination (field_total / field_map of the NeDDF kernels): samples
-// [edge0, edge0 + len) of the rays listed in ray_index[0 .. *n_active) (both NULL: rays 0, 1, ...), outputs at
-// [ray, edge] of the caller's full [n_rays, n_edges] arrays.  len = 0, as in a zero-initialised parameter block: whole
-// rows, sample n = ray n / n_edges, edge n % n_edges, outputs at n.
-struct Segment {
-  int len, edge0;
-  const int32_t* ray_index;
-  const int32_t* n_active;  // device scalar, read by the kernel: no host synchronisation between segments
-};
-
-// samples of the launch: *n_active rays of len samples, else n (the bound the grid was sized with)
-__device__ __forceinline__ int64_t seg_total(const Segment& s, int64_t n) {
-  return (s.len > 0 && s.n_active) ? (int64_t)(*s.n_active) * s.len : n;
-}
-// ray b and edge j of sample n (rays of n_edges edges)
-__device__ __forceinline__ void seg_ray_edge(const Segment& s, int n_edges, int64_t n, int64_t& b, int& j) {
-  if (s.len > 0) {
-    const int64_t r = n / s.len;
-    j = s.edge0 + (int)(n - r * s.len);
-    b = s.ray_index ? (int64_t)s.ray_index[r] : r;
-  } else {
-    b = n / n_edges;
-    j = (int)(n - b * n_edges);
-  }
-}
-// where sample n's outputs go (n itself for whole rows and for explicit samples)
-__device__ __forceinline__ int64_t seg_out(const Segment& s, int n_edges, int64_t n) {
-  if (s.len == 0) return n;
-  int64_t b;
-  int j;
-  seg_ray_edge(s, n_edges, n, b, j);
-  return b * n_edges + j;
-}
-
 // torch Linear weight [out][in] -> entry (k = input channel, c = output channel) of the forward pack [k_pad][256]
 __device__ __forceinline__ float pack_entry(const float* w, int n_in, int n_out, int k, int c) {
   return (k < n_in && c < n_out) ? w[(size_t)c * n_in + k] : 0.f;
@@ -165,8 +132,8 @@ struct Linears {
 };
 
 #ifdef __CUDACC__
-// The network part of a kernel's parameters (.w the packed weights, .n the samples): the parameters themselves, unless
-// an overload in the kernel's namespace says otherwise (neust::net).
+// The network part of a kernel's parameters (.w the packed weights, .n the samples): the parameters themselves,
+// unless an overload in the kernel's namespace says otherwise (neust::net).
 template <class Prm>
 Prm& net(Prm& P) {
   return P;
@@ -245,17 +212,6 @@ struct Handle {
 inline int32_t check_rays(const char* who, int32_t n_edges, int32_t sampling_type) {
   if (n_edges < 1 || (sampling_type != NEDDF_SAMPLING_POINT && sampling_type != NEDDF_SAMPLING_CONE))
     return fail(NEDDF_E_INVALID, std::string(who) + ": bad n_edges / sampling_type");
-  return NEDDF_OK;
-}
-
-// the segment of the _rays_segment entry points (after check_rays), into P's Segment
-inline int32_t check_segment(const char* who, int32_t n_edges, int32_t edge0, int32_t seg_len, const int32_t* ray_index,
-                             const int32_t* n_active, Segment& seg) {
-  if (edge0 < 0 || seg_len < 1 || (int64_t)edge0 + seg_len > n_edges)
-    return fail(NEDDF_E_INVALID, std::string(who) + ": bad segment (need 0 <= edge0, 1 <= seg_len, edge0 + seg_len <= n_edges)");
-  if ((ray_index == nullptr) != (n_active == nullptr))
-    return fail(NEDDF_E_INVALID, std::string(who) + ": d_ray_index and d_n_active go together");
-  seg = Segment{seg_len, edge0, ray_index, n_active};
   return NEDDF_OK;
 }
 #endif

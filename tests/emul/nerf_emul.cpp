@@ -29,10 +29,7 @@ extern "C" int nerf_emul_forward_segment(const neddf_nerf_config_t* cfg, const f
   nerf::pack(0, 1, P, t, packed.data());  // neddf_nerf_set_weights
   P.w = packed.data();
   for (int e = 0; e < cfg->embed_pos_rank; ++e) P.lowpass[e] = lowpass[e];
-  P.n = n_rays * (seg_len > 0 ? seg_len : n_edges);
-  P.ray_dir = ray_dir; P.ray_orig = ray_orig; P.dists = dists;
-  P.n_edges = n_edges; P.sampling_type = sampling_type; P.ray_radius = ray_radius;
-  P.seg = simt::Segment{seg_len, edge0, ray_index, n_active};
+  set_rays(P, ray_dir, ray_orig, dists, n_rays, n_edges, sampling_type, ray_radius, Segment{seg_len, edge0, ray_index, n_active});
   P.density = density; P.color = color;
   if (P.n <= 0) return 0;
   emul::run_grid(nblocks, nerf::kThreads, nerf::kSmemFloats, 0, [&](emul::HostCtx& cx, float* smem) { nerf::tile_program(cx, P, smem); });

@@ -24,14 +24,8 @@ static int setup(const neddf_nerf_config_t* cfg, bool training, const float* con
   nerf::pack(0, 1, P, t, packed.data());  // neddf_nerf_set_weights / neddf_nerf_train_set_weights
   P.w = packed.data();
   for (int e = 0; e < cfg->embed_pos_rank; ++e) P.lowpass[e] = lowpass[e];
-  if (dists) {
-    P.n = n * n_edges;
-    P.ray_dir = ray_dir; P.ray_orig = ray_orig; P.dists = dists;
-    P.n_edges = n_edges; P.sampling_type = sampling_type; P.ray_radius = ray_radius;
-  } else {
-    P.n = n;
-    P.pos = pos; P.dir = dir; P.var = var;
-  }
+  if (dists) set_rays(P, ray_dir, ray_orig, dists, n, n_edges, sampling_type, ray_radius);
+  else set_samples(P, n, pos, dir, var);
   return 0;
 }
 

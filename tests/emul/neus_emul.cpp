@@ -29,14 +29,8 @@ extern "C" int neus_emul_forward(const neddf_neus_config_t* cfg, const float* co
   std::vector<float> packed(w_floats, 0.f);
   neus::pack(0, 1, P, nullptr, nullptr, t, packed.data());  // neddf_neus_set_weights
   P.w = packed.data();
-  if (dists) {
-    P.n = n * n_edges;
-    P.ray_dir = ray_dir; P.ray_orig = ray_orig; P.dists = dists;
-    P.n_edges = n_edges; P.sampling_type = sampling_type; P.ray_radius = ray_radius;
-  } else {
-    P.n = n;
-    P.pos = pos; P.dir = dir;
-  }
+  if (dists) set_rays(P, ray_dir, ray_orig, dists, n, n_edges, sampling_type, ray_radius);
+  else set_samples(P, n, pos, dir, nullptr);
   P.sdf = sdf; P.density = density; P.color = color; P.normal = normal;
   if (P.n <= 0) return 0;
 #ifdef NEUS_EMUL_MISALIGN  // negative control: shared memory base off by one float (a float4 access is then misaligned)

@@ -28,10 +28,7 @@ extern "C" int neus_emul_forward_segment(const neddf_neus_config_t* cfg, const f
   std::vector<float> packed(w_floats, 0.f);
   neus::pack(0, 1, P, nullptr, nullptr, t, packed.data());  // neddf_neus_set_weights
   P.w = packed.data();
-  P.n = n_rays * (seg_len > 0 ? seg_len : n_edges);
-  P.ray_dir = ray_dir; P.ray_orig = ray_orig; P.dists = dists;
-  P.n_edges = n_edges; P.sampling_type = sampling_type; P.ray_radius = ray_radius;
-  P.seg = simt::Segment{seg_len, edge0, ray_index, n_active};
+  set_rays(P, ray_dir, ray_orig, dists, n_rays, n_edges, sampling_type, ray_radius, Segment{seg_len, edge0, ray_index, n_active});
   P.density = density; P.color = color;
   if (P.n <= 0) return 0;
   emul::run_grid(nblocks, neus::kThreads, neus::kSmemFloats, 0, [&](emul::HostCtx& cx, float* smem) { neus::tile_program(cx, P, smem); });

@@ -26,14 +26,8 @@ extern "C" int neus_train_emul(const neddf_neus_config_t* cfg, const float* cons
   neus::pack(0, 1, T.f, T.wt_sdf, T.wt_col, t, packed.data());  // neddf_neus_train_set_weights
   neus::Params& P = T.f;
   P.w = packed.data();
-  if (dists) {
-    P.n = n * n_edges;
-    P.ray_dir = ray_dir; P.ray_orig = ray_orig; P.dists = dists;
-    P.n_edges = n_edges; P.sampling_type = sampling_type; P.ray_radius = ray_radius;
-  } else {
-    P.n = n;
-    P.pos = pos; P.dir = dir;
-  }
+  if (dists) set_rays(P, ray_dir, ray_orig, dists, n, n_edges, sampling_type, ray_radius);
+  else set_samples(P, n, pos, dir, nullptr);
   T.g_sdf = g_sdf; T.g_density = g_density; T.g_color = g_color; T.g_normal = g_normal;
   T.E4 = bufs[0]; T.XS = bufs[1]; T.GS = bufs[2]; T.XC0 = bufs[3]; T.FO = bufs[4];
   T.XC = bufs[5]; T.GC = bufs[6]; T.GH = bufs[7]; T.GV = bufs[8];

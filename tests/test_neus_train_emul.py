@@ -74,8 +74,8 @@ def emul():
         pytest.skip("g++ / CUDA headers not available")
     csrc = os.path.join(HERE, "..", "neddf_b200", "csrc")
     deps = [SRC, os.path.join(HERE, "emul", "emul_common.h"), os.path.join(csrc, "neus_train_kernel.cuh"),
-            os.path.join(csrc, "neus_kernel.cuh"), os.path.join(csrc, "simt_tile.cuh"), os.path.join(csrc, "common.cuh"),
-            os.path.join(HERE, "..", "include", "neddf_b200.h")]
+            os.path.join(csrc, "neus_kernel.cuh"), os.path.join(csrc, "simt_tile.cuh"), os.path.join(csrc, "samples.cuh"),
+            os.path.join(csrc, "common.cuh"), os.path.join(HERE, "..", "include", "neddf_b200.h")]
     if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in deps):
         subprocess.run(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-pthread", "-I" + CUDA_INC, SRC, "-o", LIB],
                        check=True)

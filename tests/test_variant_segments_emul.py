@@ -44,7 +44,7 @@ def _build(src: str, lib: str, headers):
 def libs():
     if shutil.which("g++") is None or not os.path.isdir(CUDA_INC):
         pytest.skip("g++ / CUDA headers not available")
-    common = ["simt_tile.cuh", "common.cuh"]
+    common = ["simt_tile.cuh", "samples.cuh", "common.cuh"]
     nerf = _build("nerf_emul.cpp", "libnerf_emul.so", ["nerf_kernel.cuh", "field_math.cuh"] + common)
     neus = _build("neus_segment_emul.cpp", "libneus_segment_emul.so", ["neus_kernel.cuh"] + common)
     for f in (nerf.nerf_emul_forward_segment, neus.neus_emul_forward_segment):
