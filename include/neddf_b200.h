@@ -373,6 +373,36 @@ int32_t neddf_nerf_forward_rays_segment(const neddf_nerf_t* h, const float* lowp
                                         float* d_color, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * NeRF field variant on the tensor cores (engines "tc" and "auto" of neddf_b200.NeRF): one persistent wgmma kernel
+ * (csrc/nerf_tc.cu), every GEMM operand split into fp16 hi + lo with three products accumulated in fp32, the heads in
+ * fp32.  It accepts exactly the configurations neddf_nerf_create accepts, with the same codes, and every entry point
+ * takes the arguments of its neddf_nerf_* counterpart with the same checks.  An operand outside fp16 range (65504)
+ * sets bit 4 of the handle's status word (as neddf_field_status); that launch's outputs are invalid.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct neddf_nerf_tc neddf_nerf_tc_t; /* opaque: config + packed fp16 hi/lo weight chunks + status word */
+
+int32_t neddf_nerf_tc_create(const neddf_nerf_config_t* cfg, neddf_nerf_tc_t** out);
+void neddf_nerf_tc_destroy(neddf_nerf_tc_t* h);
+/* = neddf_nerf_set_weights */
+int32_t neddf_nerf_tc_set_weights(neddf_nerf_tc_t* h, const float* const* d_w, const float* const* d_b, int32_t n_layers,
+                                  void* stream);
+/* = neddf_nerf_forward */
+int32_t neddf_nerf_tc_forward(const neddf_nerf_tc_t* h, const float* lowpass, const float* d_pos, const float* d_dir,
+                              const float* d_var, int64_t n, float* d_density, float* d_color, void* stream);
+/* = neddf_nerf_forward_rays */
+int32_t neddf_nerf_tc_forward_rays(const neddf_nerf_tc_t* h, const float* lowpass, const float* d_ray_dir,
+                                   const float* d_ray_orig, const float* d_dists, int64_t n_rays, int32_t n_edges,
+                                   int32_t sampling_type, float ray_radius, float* d_density, float* d_color, void* stream);
+/* = neddf_nerf_forward_rays_segment; each evaluated entry equals neddf_nerf_tc_forward_rays' bit for bit */
+int32_t neddf_nerf_tc_forward_rays_segment(const neddf_nerf_tc_t* h, const float* lowpass, const float* d_ray_dir,
+                                           const float* d_ray_orig, const float* d_dists, int64_t n_rays, int32_t n_edges,
+                                           int32_t sampling_type, float ray_radius, int32_t edge0, int32_t seg_len,
+                                           const int32_t* d_ray_index, const int32_t* d_n_active, float* d_density,
+                                           float* d_color, void* stream);
+/* Read and clear the status word (synchronises `stream`): bit 4 = an operand left fp16 range since the last read. */
+int32_t neddf_nerf_tc_status(const neddf_nerf_tc_t* h, int32_t* h_status_out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * NeuS field variant (SURVEY 8(f) item 3; neddf/network/neus.py).  Forward only, fp32 CUDA-core kernel
  * (csrc/neus_simt.cu + csrc/neus_kernel.cuh); the normal d sdf / d position, which the reference takes with
  * torch.autograd.grad (neus.py:133-142), is carried forward through the SDF trunk as three Jacobian rows.

@@ -106,6 +106,14 @@ _SIGNATURES = {
     "neddf_nerf_forward": (_I32, [_P, _FP, _P, _P, _P, _I64, _P, _P, _P]),
     "neddf_nerf_forward_rays": (_I32, [_P, _FP, _P, _P, _P, _I64, _I32, _I32, _F, _P, _P, _P]),
     "neddf_nerf_forward_rays_segment": (_I32, [_P, _FP, _P, _P, _P, _I64, _I32, _I32, _F, _I32, _I32, _P, _P, _P, _P, _P]),
+    "neddf_nerf_tc_create": (_I32, [C.POINTER(NerfConfig), C.POINTER(_P)]),
+    "neddf_nerf_tc_destroy": (None, [_P]),
+    "neddf_nerf_tc_set_weights": (_I32, [_P, C.POINTER(_P), C.POINTER(_P), _I32, _P]),
+    "neddf_nerf_tc_forward": (_I32, [_P, _FP, _P, _P, _P, _I64, _P, _P, _P]),
+    "neddf_nerf_tc_forward_rays": (_I32, [_P, _FP, _P, _P, _P, _I64, _I32, _I32, _F, _P, _P, _P]),
+    "neddf_nerf_tc_forward_rays_segment": (_I32, [_P, _FP, _P, _P, _P, _I64, _I32, _I32, _F, _I32, _I32, _P, _P, _P, _P,
+                                                  _P]),
+    "neddf_nerf_tc_status": (_I32, [_P, C.POINTER(C.c_int32), _P]),
     "neddf_nerf_train_create": (_I32, [C.POINTER(NerfConfig), C.POINTER(_P)]),
     "neddf_nerf_train_destroy": (None, [_P]),
     "neddf_nerf_train_set_weights": (_I32, [_P, C.POINTER(_P), C.POINTER(_P), _I32, _P]),

@@ -1,6 +1,14 @@
 """Drop-in for neddf.network.NeRF (neddf/network/nerf.py:13-178) on the CUDA path: same constructor, same
 module / state_dict layout (``layers.N``, ``outL_density``, ``outL_color.0`` / ``.2``), ``forward(Sampling)`` and
-``set_iter``; the network itself runs in one CUDA kernel (``csrc/nerf_simt.cu`` behind ``neddf_nerf_*``).
+``set_iter``; the network itself runs in one CUDA kernel per engine (``NeRF.engine``, set by ``NeRFRender.set_engine``):
+
+- "fp32" (the default): ``csrc/nerf_simt.cu`` behind ``neddf_nerf_*``, every multiply-add an fp32 FMA;
+- "tc": ``csrc/nerf_tc.cu`` behind ``neddf_nerf_tc_*``, a wgmma kernel whose GEMM operands are split into fp16 hi + lo
+  (three products, fp32 accumulation; the heads in fp32).  An activation outside fp16 range raises FloatingPointError;
+- "auto": "tc", until it leaves fp16 range once; the network then raises EngineRangeError, which NeRFRender answers by
+  re-running the call, and stays on "fp32" until the next ``set_engine``.
+
+NeRF has no CTA-pair form: "tc2" runs the fp32 kernel.
 
 Scope (SURVEY 8(f) item 3): inference - ``forward`` / ``forward_rays`` under ``torch.no_grad()``, i.e. everything
 ``NeRFRender.render_image`` and ``render_rays`` in eval need.  By default a call with autograd enabled on trainable
@@ -11,6 +19,7 @@ nerf.py:107-165 with respect to the parameters runs in ``csrc/nerf_train.cu`` (f
 gradients in fp32 FMA) + ``neddf_wgrad`` / ``neddf_colsum_value_rows`` (weight / bias gradients).  That kernel has so far
 been validated through the host emulation of its tile program only (tests/test_nerf_train_emul.py: the real reference's
 autograd gradients, sanitizers) - it was written after the round's GPU budget was spent - hence the opt-in."""
+import ctypes as C
 import math
 import os
 from typing import Dict, List, Optional
@@ -20,7 +29,7 @@ from torch import Tensor, nn
 
 from . import _lib as L
 from ._host import KernelHandle, WeightGrad
-from .network import BaseNeuralField
+from .network import BaseNeuralField, EngineRangeError
 from .ray import Sampling
 
 
@@ -37,7 +46,8 @@ def lowpass_scale(embed_dim: int, alpha: float) -> List[float]:
 
 
 class _NerfTrainFn(torch.autograd.Function):
-    """NeRF.forward under autograd.  forward: the inference kernel (neddf_nerf_forward[_rays]); backward:
+    """NeRF.forward under autograd.  forward: the fp32 inference kernel (neddf_nerf_forward[_rays]) whatever the engine,
+    since the backward recomputes that kernel's tile program and must differentiate the values it returned; backward:
     neddf_nerf_train_backward[_rays] (recomputes the forward per tile, leaves layer inputs X and pre-activation gradients
     G in global memory), then gW = X^T G as tensor-core split-K GEMMs (neddf_wgrad) and bias gradients as column sums.
     Gradients flow to the module's parameters only (nerf_trainer.py:38-42 optimises nothing else)."""
@@ -113,7 +123,7 @@ class _NerfTrainFn(torch.autograd.Function):
 
 class NeRF(BaseNeuralField):
     _MESH_VIEW_SIGN = {"density": 1.0}  # density grows inward
-    _HANDLES = (KernelHandle("neddf_nerf"), KernelHandle("neddf_nerf_train", "_train"))
+    _HANDLES = (KernelHandle("neddf_nerf"), KernelHandle("neddf_nerf_train", "_train"), KernelHandle("neddf_nerf_tc", "_tc"))
     _GRAD_REFUSAL = (
         "neddf_b200.NeRF is forward-only on the CUDA path by default: wrap the call in torch.no_grad() / use "
         "render_image, or train with the reference and load the checkpoint.  The training backward kernel "
@@ -152,7 +162,8 @@ class NeRF(BaseNeuralField):
         self.lowpass_alpha_offset = float(lowpass_alpha_offset)
         self.lowpass_alpha = float(lowpass_alpha_offset)
         # kernel-side state
-        self.engine = "fp32"  # the only engine of this variant; NeRFRender.set_engine may overwrite the attribute
+        self.engine = "fp32"          # "fp32" | "tc" | "auto" ("tc2": fp32, no pair form); NeRFRender.set_engine sets it
+        self._range_fallback = False  # "auto" met an activation outside fp16 range: it resolves to fp32 from then on
         # training backward (csrc/nerf_train.cu): opt-in until it has been run on hardware (module docstring)
         self.training_kernels = os.environ.get("NEDDF_NERF_TRAIN", "0") not in ("", "0")
 
@@ -172,10 +183,44 @@ class NeRF(BaseNeuralField):
         return self._fill_skips(c)
 
     def _launch_forward(self, a: Tensor, b: Tensor, c: Tensor, sampling_type, ray_radius: float) -> Dict[str, Tensor]:
-        """The inference kernels on rays (sampling_type given) or explicit samples; called under no_grad."""
+        """The fp32 inference kernel, whatever the engine (the training backward recomputes it), on rays (sampling_type
+        given) or explicit samples; called under no_grad."""
         if sampling_type is not None:
-            return self.forward_rays(a, b, c, sampling_type, ray_radius)
-        return self.forward(Sampling(a, b, c))
+            return self.forward_rays(a, b, c, sampling_type, ray_radius, _engine="fp32")
+        return self.forward(Sampling(a, b, c), _engine="fp32")
+
+    def resolved_engine(self, device=None) -> str:
+        """Engine whose kernel the next inference call runs: "tc" for "tc", and for "auto" until it has left fp16
+        range; "fp32" otherwise (NeRF has no pair form: "tc2" runs the fp32 kernel)."""
+        if self.engine == "tc" or (self.engine == "auto" and not self._range_fallback):
+            return "tc"
+        return "fp32"
+
+    def _kernel(self, device: torch.device, engine: Optional[str]):
+        """(handle, ABI prefix) of the inference kernel of ``engine`` (None: ``resolved_engine()``)."""
+        if (engine or self.resolved_engine()) == "tc":
+            return self._field(device, kind=2), "neddf_nerf_tc"
+        return self._field(device), "neddf_nerf"
+
+    def check_engine_status(self) -> None:
+        """Read-and-clear the tensor-core kernel's device status word (one sync).  Raises if it met an activation
+        outside fp16 range (its operands are fp16 hi+lo pairs): EngineRangeError once under "auto", which then resolves
+        to the fp32 kernel; FloatingPointError under "tc"."""
+        if getattr(self, "_tc_handle", None) is None:
+            return
+        v = C.c_int32(0)
+        dev = self._tc_handle_device
+        with torch.cuda.device(dev):
+            L.check(L.lib().neddf_nerf_tc_status(self._tc_handle, C.byref(v), L.stream_ptr(dev)), "nerf_tc_status")
+        if v.value & 4:
+            if self.engine == "auto" and not self._range_fallback:
+                self._range_fallback = True
+                raise EngineRangeError(
+                    "neddf_b200: tensor-core engine saw |activation| > 65504 (fp16 range of its split operands); "
+                    "engine 'auto' now resolves to the fp32 engine for this network and the call is re-run")
+            raise FloatingPointError(
+                "neddf_b200: tensor-core engine saw |activation| > 65504 (fp16 range of its split operands); "
+                "results of the last calls are invalid - use set_engine('fp32') or 'auto' for this network")
 
     def _forward_autograd(self, a: Tensor, b: Tensor, c: Tensor, sampling_type, ray_radius: float) -> Dict[str, Tensor]:
         density, color = _NerfTrainFn.apply(self, a, b, c, sampling_type, float(ray_radius), *self._param_tensors())
@@ -185,7 +230,7 @@ class NeRF(BaseNeuralField):
         return L.fbuf(lowpass_scale(self.embed_pos_rank, self.lowpass_alpha))
 
     # ----------------------------------------------------------------------- forward --
-    def forward(self, sampling: Sampling) -> Dict[str, Tensor]:
+    def forward(self, sampling: Sampling, _engine: Optional[str] = None) -> Dict[str, Tensor]:
         """nerf.py:107-165: {'density': [B,S], 'color': [B,S,3]}."""
         pos = L.require_cuda_f32(sampling.sample_pos, "sample_pos")
         sdir = L.require_cuda_f32(sampling.sample_dir, "sample_dir")
@@ -196,15 +241,16 @@ class NeRF(BaseNeuralField):
         device = pos.device
         out = {"density": torch.empty(B, S, device=device, dtype=torch.float32),
                "color": torch.empty(B, S, 3, device=device, dtype=torch.float32)}
-        h = self._field(device)
+        h, pre = self._kernel(device, _engine)
         with torch.cuda.device(device):
-            L.check(L.lib().neddf_nerf_forward(h, self._lowpass(), L.ptr(pos), L.ptr(sdir), L.ptr(var), B * S,
-                                               L.ptr(out["density"]), L.ptr(out["color"]), L.stream_ptr(device)),
-                    "nerf_forward")
+            L.check(getattr(L.lib(), pre + "_forward")(h, self._lowpass(), L.ptr(pos), L.ptr(sdir), L.ptr(var), B * S,
+                                                       L.ptr(out["density"]), L.ptr(out["color"]), L.stream_ptr(device)),
+                    pre[len("neddf_"):] + "_forward")
         return out
 
     def forward_rays(self, ray_dir: Tensor, ray_orig: Tensor, dists: Tensor, sampling_type: str, ray_radius: float,
-                     need_penalty: bool = True, need_aux: bool = True, need_color: bool = True) -> Dict[str, Tensor]:
+                     need_penalty: bool = True, need_aux: bool = True, need_color: bool = True,
+                     _engine: Optional[str] = None) -> Dict[str, Tensor]:
         """Same network with the sample geometry fused into the kernel (what NeRFRender calls; the NeRF variant has
         neither penalties nor auxiliary fields, the flags are accepted for interface parity)."""
         ray_dir = L.require_cuda_f32(ray_dir, "ray_dir")
@@ -216,11 +262,12 @@ class NeRF(BaseNeuralField):
         device = dists.device
         out = {"density": torch.empty(B, S, device=device, dtype=torch.float32),
                "color": torch.empty(B, S, 3, device=device, dtype=torch.float32)}
-        h = self._field(device)
+        h, pre = self._kernel(device, _engine)
         with self._profiled(device, B * S), torch.cuda.device(device):
-            L.check(L.lib().neddf_nerf_forward_rays(h, self._lowpass(), L.ptr(ray_dir), L.ptr(ray_orig), L.ptr(dists), B, S,
-                                                    L.SAMPLING_IDS[sampling_type], float(ray_radius), L.ptr(out["density"]),
-                                                    L.ptr(out["color"]), L.stream_ptr(device)), "nerf_forward_rays")
+            L.check(getattr(L.lib(), pre + "_forward_rays")(
+                h, self._lowpass(), L.ptr(ray_dir), L.ptr(ray_orig), L.ptr(dists), B, S, L.SAMPLING_IDS[sampling_type],
+                float(ray_radius), L.ptr(out["density"]), L.ptr(out["color"]), L.stream_ptr(device)),
+                pre[len("neddf_"):] + "_forward_rays")
         return out
 
     def forward_rays_segment(self, ray_dir: Tensor, ray_orig: Tensor, dists: Tensor, sampling_type: str, ray_radius: float,
@@ -233,13 +280,13 @@ class NeRF(BaseNeuralField):
         self._refuse_autograd("forward_rays_segment")
         B, E = dists.shape
         device = dists.device
-        h = self._field(device)
+        h, pre = self._kernel(device, None)
         # the executed count lives on the device (NeRFRender.termination_stats): no n_evaluations
         with self._profiled(device, None), torch.cuda.device(device):
-            L.check(L.lib().neddf_nerf_forward_rays_segment(
+            L.check(getattr(L.lib(), pre + "_forward_rays_segment")(
                 h, self._lowpass(), L.ptr(ray_dir), L.ptr(ray_orig), L.ptr(dists), B, E, L.SAMPLING_IDS[sampling_type],
                 float(ray_radius), int(edge0), int(seg_len), L.ptr(ray_index), L.ptr(n_active), L.ptr(density), L.ptr(color),
-                L.stream_ptr(device)), "nerf_forward_rays_segment")
+                L.stream_ptr(device)), pre[len("neddf_"):] + "_forward_rays_segment")
 
     def set_iter(self, iter: int) -> None:
         """nerf.py:167-178."""

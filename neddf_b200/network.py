@@ -189,12 +189,13 @@ class BaseNeuralField(nn.Module):
             h.reset(self)
         self._profile_events = None  # bench.py: list receiving (start, end, n_evaluations or None) CUDA events
 
-    def _field(self, device: torch.device):
-        """Forward handle with weights packed for the parameters' current values."""
+    def _field(self, device: torch.device, kind: int = 0):
+        """Forward handle (``_HANDLES[kind]``: another inference kernel of the network) with weights packed for the
+        parameters' current values."""
         if device.type != "cuda":
             raise RuntimeError(f"neddf_b200.{type(self).__name__} runs on CUDA devices only: move the module with "
                                ".to('cuda') (the hot path has no CPU implementation)")
-        return self._HANDLES[0].get(self, device)
+        return self._HANDLES[kind].get(self, device)
 
     def _train_field(self, device: torch.device):
         """Handle of the training-backward kernel (NeRF, NeuS), re-packed like ``_field``'s."""

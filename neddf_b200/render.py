@@ -320,7 +320,8 @@ class NeRFRender(BaseNeuralRender):
         self.network_fine.set_iter(iter)
 
     def set_engine(self, engine: str) -> None:
-        """"auto" | "fp32" (CUDA-core fp32 FMA) | "tc" (wgmma, split-fp16 operands) | "tc2" (the same kernel in CTA pairs)."""
+        """"auto" | "fp32" (CUDA-core fp32 FMA) | "tc" (wgmma, split-fp16 operands) | "tc2" (the same kernel in CTA pairs).
+        NeRF has "fp32", "tc" and "auto" ("tc2" runs its fp32 kernel); NeuS runs its fp32 kernel under every engine."""
         if engine not in L.ENGINE_IDS:
             raise ValueError(engine)
         for net in (self.network_fine, self.network_coarse):
